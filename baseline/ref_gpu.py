@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""Reference GPU arm: the UNMODIFIED reference engine (tanishqkumar/ssd, installed under baseline/_ref by
-`__graft_entry__.build()` with `pip install --no-deps --target baseline/_ref /root/reference`) driven through its own public
+"""Reference GPU arm: the UNMODIFIED reference engine (tanishqkumar/ssd, installed under oracle/_ref by
+`__graft_entry__.build()` from the reference checkout, oracle/reference_build.py) driven through its own public
 API — `ssd.LLM(...)`, `add_request`, `create_inference_step`, `step` — on this box's GPU: its `LlamaForCausalLM` /
 `Qwen3ForCausalLM`, `F.linear` (cuBLAS), its `@torch.compile` regions (Inductor -> Triton), its Triton `store_kvcache`,
 its CUDA-graph capture / replay (`capture_cudagraph`, `run_decode_cudagraph`, `run_verify_cudagraph`), its `Sampler`,
@@ -8,7 +8,7 @@ its CUDA-graph capture / replay (`capture_cudagraph`, `run_decode_cudagraph`, `r
 
 What has to be supplied from outside, because the image is not the reference's pinned environment (SURVEY §7/§8c):
   1. `sgl_kernel.flash_attn` (FA3 wheel, absent, Hopper-only): two functions backed by flash_attn 2.8.3, which ships
-     sm_100 SASS — the stub BASELINE.md §4.2 prescribes;
+     sm_90 SASS — the stub BASELINE.md §4.2 prescribes;
   2. checkpoints: none exist in the image, so `ssd.engine.model_runner.load_model` is replaced by a filler that writes
      ssd_b200.synth's seeded synthetic weights (the same tensors our engine runs on) into the reference's own
      nn.Parameters, and `AutoTokenizer.from_pretrained` returns the synthetic "<id>" tokenizer for synthetic dirs;
@@ -32,7 +32,7 @@ import types
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
-REF_DIR = os.path.join(HERE, "_ref")
+REF_DIR = os.path.join(ROOT, "oracle", "_ref")
 
 
 def install_flash_attn_stub():
@@ -68,11 +68,11 @@ def install_flash_attn_stub():
 
 def import_reference():
     if not os.path.isdir(os.path.join(REF_DIR, "ssd")):
-        raise RuntimeError(f"{REF_DIR}/ssd missing: run `python -c 'import __graft_entry__ as g; g.build()'` in the build "
-                           "container (pip install --no-deps --target baseline/_ref /root/reference)")
+        raise RuntimeError(f"{REF_DIR}/ssd missing: run `python -c 'import __graft_entry__ as g; g.build()'` with "
+                           "a reference checkout (oracle/reference_build.py; SSD_REFERENCE_DIR overrides its location)")
     os.environ.setdefault("SSD_HF_CACHE", tempfile.gettempdir())
     os.environ.setdefault("SSD_DATASET_DIR", tempfile.gettempdir())
-    os.environ.setdefault("SSD_CUDA_ARCH", "10.0")
+    os.environ.setdefault("SSD_CUDA_ARCH", "9.0")
     for mod in [k for k in sys.modules if k == "ssd" or k.startswith("ssd.")]:
         del sys.modules[mod]
     sys.path.insert(0, REF_DIR)
@@ -84,7 +84,7 @@ def import_reference():
         w = types.ModuleType("wandb")
         w.init = w.log = w.finish = lambda *a, **k: None
         sys.modules["wandb"] = w
-    import ssd  # noqa: F401  (the reference package; baseline/_ref is first on sys.path)
+    import ssd  # noqa: F401  (the reference package; oracle/_ref is first on sys.path)
     assert os.path.realpath(os.path.dirname(ssd.__file__)).startswith(os.path.realpath(REF_DIR)), ssd.__file__
     return ssd
 
@@ -218,7 +218,7 @@ def run(args) -> dict:
            "dtype": "bf16", "data": "synthetic", "accept_len": sum(lens) / max(1, len(lens)),
            "config": {"workload": f"{desc}, sync SD k={K} b=1 temp={temp:g}, TP=1, prompt {args.prompt_len} random tokens, "
                                   f"synthetic bigram-agreement weights alpha={args.alpha} — UNMODIFIED reference engine "
-                                  f"(baseline/_ref) on the GPU: F.linear/cuBLAS, torch.compile, its CUDA graphs, "
+                                  f"(oracle/_ref) on the GPU: F.linear/cuBLAS, torch.compile, its CUDA graphs, "
                                   f"flash_attn 2.8.3 behind the sgl_kernel.flash_attn stub",
                       "enforce_eager": bool(args.eager), "init_s": round(init_s, 1), "torch": torch.__version__},
            "e2e": {"value": toks / dt, "unit": "tokens/s", "h2d_bytes_per_step": None, "d2h_bytes_per_step": None},

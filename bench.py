@@ -2,17 +2,17 @@
 """bench.py — decode tokens/s of the sync speculative-decoding hot path (BASELINE.json metric).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference|reference-gpu]
-                    [--workload 70b|8b|qwen32b|tiny] [--temp T] [--lm-scale S]
+                    [--workload 8b|70b|qwen32b|tiny] [--temp T] [--lm-scale S] [--dump-outputs DIR]
 
 A "step" is one pass of the hot path over one batch: K_spec+1 draft forwards -> one (K_spec+1)-token target
-forward -> accept/reject+resample.  Workload (N=1 default): Llama-3.1-70B target + Llama-3.2-1B draft, k=6, b=1,
-temp 0, synthetic "bigram agreement" weights at the exact shapes (there are no checkpoints in the image), random
+forward -> accept/reject+resample.  Workload (default): Llama-3.1-8B target + Llama-3.2-1B draft, k=6, b=1,
+temp 0 (17.5 GB of bf16 weights: fits one 80 GB H100; the 70B target's 139 GB needs --gpus 4), synthetic "bigram agreement" weights at the exact shapes (there are no checkpoints in the image), random
 128-token prompt.  Prints ONE JSON line (rank 0):
 
   value     decode tokens/s, device-resident loop (inputs already in HBM; CUDA events; max over ranks)
   e2e       the same metric through the public engine API (LLMEngine.step: scheduler + ssdk_spec_step with HOST
             buffers: per-step H2D of ctx/recovery/block tables and D2H of tokens/accept count inside the timing)
-  roofline  achieved HBM GB/s of the dominant kernel (weight-streaming tcgen05 GEMM, largest instance) vs the
+  roofline  achieved HBM GB/s of the dominant kernel (weight-streaming wgmma GEMM, largest instance) vs the
             measured peak, plus the whole-step fraction of the HBM roofline of SURVEY §8(d)
   cpu_baseline  the oracle (CPU restatement of the reference path) timed on the host cores on a bounded sample
   parity_check  temp 0: the tokens of the timed device-resident loop AND of the engine (e2e) loop against the closed-form
@@ -56,7 +56,7 @@ def measured_peaks():
         with open(p) as f:
             d = json.load(f)
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (not measured)"
 
 
 class ClockSampler:
@@ -169,7 +169,7 @@ def run_ours(args):
     max_len = max(4096, -(-need // 256) * 256)
     ref_gpu = None
     if world == 1 and not args.no_ref_gpu and args.workload != "tiny":
-        ref_gpu = run_reference_gpu_subprocess(args)  # BEFORE our engine takes the GPU memory (70B: 141 GB each)
+        ref_gpu = run_reference_gpu_subprocess(args)  # BEFORE our engine takes the GPU memory (both hold the weights)
     tdir = synth.make_model_dir(root, tshape, "target", seed=0, alpha=args.alpha, lm_scale=args.lm_scale)
     ddir = synth.make_model_dir(root, dshape, "draft", seed=0, alpha=args.alpha, lm_scale=args.lm_scale)
     temp = float(args.temp)
@@ -200,6 +200,7 @@ def run_ours(args):
         runner.step_resident(1)
     sync_all()
     _, tot0, _ = runner.fetch(1)
+    log0 = len(runner.resident_log(0))  # tokens the warm-up steps emitted
     l0 = runner.launch_count
     with ClockSampler(local) as cs:
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -210,8 +211,10 @@ def run_ours(args):
         e1.record()
         sync_all()
     ms_dev = e0.elapsed_time(e1)
-    _, tot1, _ = runner.fetch(1)
+    last_toks, tot1, last_rec = runner.fetch(1)
     dev_log = runner.resident_log(0)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, runner, last_toks, tot1, last_rec, dev_log[log0:])
     launches = runner.launch_count - l0
     toks_dev = int(tot1[0] - tot0[0])
     if world > 1:
@@ -346,16 +349,22 @@ def gemm_roofline(runner, peak):
     nbytes = w.numel() * 2
     ach = nbytes / (ms * 1e-3) / 1e9
     name = f"gemm_ws_kernel<16,EPI_SILU> gate|up [{w.shape[0]}x{w.shape[1]}] M={M}"
-    traffic = None  # dram__bytes_read+write of the same launch from the committed ncu --set full capture, if it matches
-    try:
-        with open(os.path.join(ROOT, "profiles", "gemm_traffic.json")) as f:
-            t = json.load(f)
-        if t["kernel"] == name:
-            traffic = t["dram_bytes_read"] + t["dram_bytes_write"]
-    except Exception:
-        pass
-    return {"bound": "hbm", "kernel": name, "achieved": ach, "unit": "GB/s", "frac": ach / peak, "traffic": traffic,
-            "launch_ms": ms, "bytes_per_launch": nbytes}
+    return {"bound": "hbm", "kernel": name, "achieved": ach, "unit": "GB/s", "frac": ach / peak, "launch_ms": ms,
+            "bytes_per_launch": nbytes}
+
+
+def dump_outputs(out_dir, runner, toks, total, rec, log):
+    """What the device-resident loop hands a caller after its last timed step, as float32 / float64 .npy files: the
+    step's speculations, accepted-token total and recovery token (token ids exact in float64), the target's verify
+    logits and the draft's logits of that step (bf16 values, exact in float32), and every token the timed steps emitted."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"speculations": np.asarray(toks, dtype=np.float64), "accepted_total": np.asarray(total, dtype=np.float64),
+              "recovery": np.asarray(rec, dtype=np.float64), "emitted_tokens": np.asarray(log, dtype=np.float64),
+              "target_logits": runner.logits_p(1).float().cpu().numpy(),
+              "draft_logits": runner.logits_q(1).float().cpu().numpy()}
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
 
 
 # ---------------------------------------------------------------------------------------- CPU baseline
@@ -457,12 +466,14 @@ def main():
     ap.add_argument("--temp", type=float, default=0.0, help="sampling temperature of target and draft (BASELINE config 4: 0.7)")
     ap.add_argument("--lm-scale", type=float, default=None, help="synthetic lm_head scale (softens the distribution for temp>0)")
     ap.add_argument("--no-ref-gpu", action="store_true", help="skip the reference GPU arm inside the default line")
-    ap.add_argument("--workload", default="70b", choices=sorted(WORKLOADS))
+    ap.add_argument("--workload", default="8b", choices=sorted(WORKLOADS))
     ap.add_argument("--spec-k", type=int, default=6)
     ap.add_argument("--alpha", type=float, default=0.85)
     ap.add_argument("--prompt-len", type=int, default=128)
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-pdl", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs to DIR/<name>.npy (same arguments -> same inputs)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
     if args.impl == "reference":

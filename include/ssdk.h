@@ -1,5 +1,5 @@
 /*
- * ssdk.h — C-ABI of libssdk.so, the sm_100a speculative-decoding hot path.
+ * ssdk.h — C-ABI of libssdk.so, the sm_90a (H100) speculative-decoding hot path.
  *
  * The reference (tanishqkumar/ssd) has no native code and no FFI: its hot path is
  * Python/torch calling cuBLAS, torch.compile(Triton), FlashAttention-3, FlashInfer
@@ -191,8 +191,8 @@ int64_t ssdk_launch_count(ssdk_handle h);
 
 /* ---- stand-alone ops (parity tests call these through the same C-ABI) ------ */
 
-/* y[M,N] = x[M,K] · w[N,K]^T  (bf16 in, fp32 accumulate in TMEM, bf16 out),
- * M <= 64: weight-streaming tcgen05 GEMM with TMA-fed 128B-swizzled smem tiles.
+/* y[M,N] = x[M,K] · w[N,K]^T  (bf16 in, fp32 accumulate in registers, bf16 out),
+ * M <= 64: weight-streaming wgmma GEMM with TMA-fed 128B-swizzled smem tiles.
  * Replaces F.linear at layers/linear.py:98,196 and embed_head.py:95,111.
  * split_k = 0 lets the library choose; `partials` (fp32 [split_k, M, N]) is only
  * needed when split_k != 1.  When split_k > 1 the result is left in `partials`

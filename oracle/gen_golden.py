@@ -1,4 +1,5 @@
-"""Generate tests/golden/*.npz by importing and running the UNMODIFIED reference (/root/reference).
+"""Generate tests/golden/*.npz by importing and running the UNMODIFIED reference (a checkout
+named by SSD_REFERENCE_DIR).
 
 Runs only in the build container (the reference does not travel to the GPU box).  Usage:
 
@@ -25,7 +26,7 @@ import torch
 REPO = Path(__file__).resolve().parent.parent
 sys.path.insert(0, str(REPO))
 OUT = REPO / "tests" / "golden"
-REF = "/root/reference"
+REF = os.environ["SSD_REFERENCE_DIR"]
 
 
 # ----------------------------------------------------------------------------- stubs
@@ -438,12 +439,12 @@ def gen_trace(ssd, family):
                prompt1=np.array(prompts[1]), rec0=np.array(rec0), spec=np.stack(steps_tokens),
                nacc=np.array(steps_nacc, dtype=np.int32), final_recovery=np.array(recovery),
                prefill_logits=lg.view(torch.int16).numpy(), **first)
-    for name, wts in (("t", wt), ("d", wd)):
-        for kname in ("embed", "lm_head", "final_norm"):
-            npz[f"{name}_{kname}"] = wts[kname].view(torch.int16).numpy()
-        for l, lw in enumerate(wts["layers"]):
-            for kname, v in lw.items():
-                npz[f"{name}_l{l}_{kname}"] = v.view(torch.int16).numpy()
+    # the draft's weights are a subset of the target's (tests/helpers.py:trace_weights rebuilds them)
+    for kname in ("embed", "lm_head", "final_norm"):
+        npz[f"t_{kname}"] = wt[kname].view(torch.int16).numpy()
+    for l, lw in enumerate(wt["layers"]):
+        for kname, v in lw.items():
+            npz[f"t_l{l}_{kname}"] = v.view(torch.int16).numpy()
     np.savez_compressed(OUT / f"trace_{family}.npz", **npz)
     print(f"trace_{family} ok; accept lens per step: {steps_nacc}")
 

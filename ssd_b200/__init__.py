@@ -1,4 +1,4 @@
-"""ssd_b200 — B200-native sync speculative-decoding hot path behind the `ssd` API surface.
+"""ssd_b200 — H100-native sync speculative-decoding hot path behind the `ssd` API surface.
 
     from ssd_b200 import LLM, SamplingParams          # same call signatures as `from ssd import ...`
     import ssd_b200.compat; ssd_b200.compat.install()  # makes `import ssd` resolve to this package

@@ -1,4 +1,4 @@
-"""Build libssdk.so (the C-ABI hot path) in-tree with nvcc for sm_100a.
+"""Build libssdk.so (the C-ABI hot path) in-tree with nvcc for sm_90a (H100).
 
     python -m ssd_b200.build            # build if stale
     python -m ssd_b200.build --force
@@ -21,7 +21,7 @@ OUT_DIR = ROOT / "_lib"
 LIB = OUT_DIR / "libssdk.so"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "-Xptxas=-v",
     "-Xcompiler", "-fPIC,-O2,-Wall,-Wno-unused-function",

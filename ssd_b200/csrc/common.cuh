@@ -1,5 +1,5 @@
-// common.cuh — shared device helpers for the sm_100a kernels of libssdk.
-// PTX wrappers (mbarrier, TMA, tcgen05/TMEM, PDL), bf16 helpers, reductions, Philox.
+// common.cuh — shared device helpers for the sm_90a kernels of libssdk.
+// PTX wrappers (mbarrier, TMA, wgmma, PDL), bf16 helpers, reductions, Philox.
 #pragma once
 // SSDK_HOST_EMU: the kernels that use no tensor-core / TMA / PTX-only feature can be compiled for the host by the test
 // suite (tests/emu/cuda_emu.h supplies the CUDA vocabulary before this header is included); never defined in the product.
@@ -205,69 +205,60 @@ SSDK_DEVINL void bulk_load_g2s(void* smem_dst, const void* gsrc, uint32_t bytes,
 }
 
 // ----------------------------------------------------------------------------------
-// PTX: tcgen05 (5th-gen tensor cores) + TMEM
+// PTX: wgmma (Hopper warpgroup MMA), both operands from shared memory
 // ----------------------------------------------------------------------------------
-SSDK_DEVINL void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-}
-SSDK_DEVINL void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-SSDK_DEVINL void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-SSDK_DEVINL void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-SSDK_DEVINL void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+SSDK_DEVINL void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+SSDK_DEVINL void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+SSDK_DEVINL void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
 
-// D[tmem] (+)= A[smem desc] * B[smem desc], kind::f16 (bf16 x bf16 -> fp32)
-SSDK_DEVINL void umma_bf16_ss(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive on an mbarrier once all previously issued tcgen05.mma of this thread retire
-SSDK_DEVINL void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// 32 lanes x 16 consecutive 32-bit columns -> 16 registers per thread
-SSDK_DEVINL void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-SSDK_DEVINL void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// Shared-memory matrix descriptor (cute::UMMA::SmemDescriptor layout), K-major operand,
-// 128-byte swizzle: 8-row x 128 B swizzle atoms stacked every 1024 B (SBO), LBO unused.
-SSDK_DEVINL uint64_t make_umma_desc_k128(const void* smem_tile) {
+// Shared-memory matrix descriptor (sm_90 GMMA layout), K-major operand, 128-byte swizzle:
+// 8-row x 128 B swizzle atoms stacked every 1024 B (SBO), LBO unused.
+SSDK_DEVINL uint64_t make_wgmma_desc_k128(const void* smem_tile) {
   const uint32_t addr = smem_u32(smem_tile);
   uint64_t d = 0;
   d |= (uint64_t)((addr >> 4) & 0x3FFFu);  // start address, bits [0,14)
   d |= (uint64_t)1u << 16;                 // leading byte offset (ignored for SW128 K-major), bits [16,30)
   d |= (uint64_t)(1024u >> 4) << 32;       // stride byte offset = 1024 B, bits [32,46)
-  d |= (uint64_t)1u << 46;                 // descriptor version = 1 (sm_100)
-  d |= (uint64_t)2u << 61;                 // layout type SWIZZLE_128B
+  d |= (uint64_t)1u << 62;                 // layout type SWIZZLE_128B, bits [62,64)
   return d;
 }
-// Instruction descriptor (cute::UMMA::InstrDescriptor layout) for kind::f16,
-// A=B=bf16 (K-major), D=fp32, dense.
-SSDK_DEVINL constexpr uint32_t make_umma_idesc_bf16(int M, int N) {
-  return (1u << 4)                      // c_format = F32
-         | (1u << 7)                    // a_format = BF16
-         | (1u << 10)                   // b_format = BF16
-         | (0u << 15) | (0u << 16)      // a_major = K, b_major = K
-         | ((uint32_t)(N >> 3) << 17)   // n_dim
-         | ((uint32_t)(M >> 4) << 24);  // m_dim
+
+// D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, A and B K-major bf16 in shared memory, D fp32 in registers of the
+// warpgroup: thread t (warp w = t / 32 of the group, lane l) holds rows 16w + l/4 + {0, 8} and columns 8c + 2(l%4) + {0, 1}
+// as d[4c + 2 * (row half) + column parity].  accumulate == 0 overwrites D.
+template <int N>
+SSDK_DEVINL void wgmma_bf16_ss(float* d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate);
+template <> SSDK_DEVINL void wgmma_bf16_ss<16>(float* d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate)
+      : "memory");
+}
+template <> SSDK_DEVINL void wgmma_bf16_ss<32>(float* d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate)
+      : "memory");
+}
+template <> SSDK_DEVINL void wgmma_bf16_ss<64>(float* d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, "
+      "%19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate)
+      : "memory");
 }
 
 // ----------------------------------------------------------------------------------

@@ -1,20 +1,20 @@
 // draft_stream.cuh — the whole speculate phase of a sync-SD step (SpeculatorSync.speculate, engine/speculator_sync.py:25-69:
 // K+1 single-token draft forwards + K samplings) as ONE persistent kernel, batch 1.
 //
-// Why: the 1B draft streams 2.47 GB per forward (0.376 ms at the measured HBM peak) but the kernel-per-op path needs
-// 0.79 ms — nine kernel boundaries per layer, during each of which HBM idles (profiles/r01_small_kernels.md).  The weights
+// Why: the 1B draft streams 2.47 GB per forward, but the kernel-per-op path has nine kernel boundaries per layer, during
+// each of which HBM idles.  The weights
 // do not depend on the activations, so here every CTA (one per SM) streams ITS share of every matrix, in program order
 // and without ever waiting for a phase, through a ring of 32 KB shared-memory slots:
 //   * a PRODUCER warp requests slot after slot with bulk async copies (cp.async.bulk global -> shared, mbarrier
 //     transaction counts, L2 evict-first) as soon as the consumers release them — across phase and layer boundaries, so
-//     while the CTAs meet at a device-wide barrier or recompute a norm the ring (148 x 160 KB = 23 MB on chip) fills with
+//     while the CTAs meet at a device-wide barrier or recompute a norm the ring (132 x 160 KB = 21 MB on chip) fills with
 //     the NEXT phases' weights;
 //   * 8 CONSUMER warps run the phases.  A projection at one token is a GEMV: each warp keeps its 64-float slice of x in
 //     registers for the whole phase and owns whole rows (K <= 2048: no cross-warp traffic at all), reads 16 bytes per
 //     lane per step from the slot (conflict-free), and releases the slot with one mbarrier arrive per warp.
-// History (profiles/r02_draft_stream.md): persistent kernel with weights read straight from global memory 0.85 ms per
-// forward; first ring version (thread 0 issuing the copies between block-wide barriers, x read from shared memory)
-// 1.05-1.15 ms: the consume loop, not HBM, was the bottleneck (1.2 us per 32 KB slot against 0.73 us of HBM time).
+// History: a persistent kernel with weights read straight from global memory was no faster than the kernel-per-op path;
+// a first ring version (thread 0 issuing the copies between block-wide barriers, x read from shared memory) was bound by
+// the consume loop, not HBM.
 //
 // Program order per forward (the five dependent stages of the reference's decoder layer, models/llama3.py:185-199):
 //   A  [residual add + input RMSNorm, recomputed by every CTA] -> q|k|v rows
@@ -99,7 +99,7 @@ SSDK_DEVINL void ds_sync() {
 // has arrived, so every CTA computes the same base).  Arrival = one release-add without a return value; waiting = relaxed
 // polling loads + one acquire fence at the end.  (A first version — acq_rel fetch-adds for arrival, counter reset and
 // generation bump, acquire loads for polling — compiled to MEMBAR.ALL.GPU + ATOMG + CCTL.IVALL three times in a row on the
-// last arriver and an L1 invalidation per poll: 2.9 us per barrier, 15 us per layer; profiles/r02_draft_stream.md.)
+// last arriver and an L1 invalidation per poll.)
 // ---------------------------------------------------------------------------------------------
 struct DsGridBar {
   unsigned long long* counter;
@@ -192,7 +192,7 @@ SSDK_DEVINL void ds_cursor_settle(const DsParams& p, const DsGeom* geom, DsCurso
 
 // the producer: one lane walks the job sequence of this CTA and refills slots as the consumers release them.  (An L2
 // window beyond the ring — `cp.async.bulk.prefetch.L2` of the next jobs, continuously or only while every requested copy
-// had landed — was measured twice and removed: 8B + 1B 8.53 / 8.63 vs 8.34 / 8.48 ms per step, profiles/r02_draft_stream.md.)
+// had landed — made the step slower and was removed.)
 SSDK_DEVINL void ds_cursor_next(const DsParams& p, const DsGeom* geom, DsCursor& c) {
   c.s += (int)gridDim.x;
   if (c.s >= geom[c.m].nj) ds_cursor_settle(p, geom, c);

@@ -130,7 +130,7 @@ static int num_sms() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
-    if (g_num_sms <= 0) g_num_sms = 148;
+    if (g_num_sms <= 0) g_num_sms = 132;
   }
   return g_num_sms;
 }
@@ -438,8 +438,8 @@ struct Fwd {
 static int attn_plan(const Model& m, int B, int Q, int* TQ, int* MT, int* nqt, int* nsplit, int max_ctx) {
   const int G = m.H / m.KV;
   if (G < 1 || G > 16 || (m.H % m.KV) != 0) return fail("unsupported GQA ratio %d", G);
-  // q tile of <= 32 rows (two 16-row MMA tiles, 8 warps = 4 token slices each): measured 7.3 us per 70B verify layer
-  // against 8.1 us with one 56-row tile and 9.5 us with 16-row tiles (profiles/r01_small_kernels.md)
+  // q tile of <= 32 rows (two 16-row MMA tiles, 8 warps = 4 token slices each): faster per verify layer than one 56-row
+  // tile or 16-row tiles
   int tq = std::min(Q, std::max(1, 32 / G));
   int R = G * tq;
   int mt = (R + 15) / 16;
@@ -590,11 +590,9 @@ static PublishParams publish_params(ssdk_engine* e, int call_idx) {
   pb.rank = m.cfg.tp_rank;
   return pb;
 }
-// SSDK_FUSED_PUBLISH=1: the row-parallel GEMM publishes from its own epilogue (EPI_PUBLISH).  Off by default: measured on
-// B200 with Llama-3.1-70B it is slower than GEMM -> ar_publish_kernel at TP=2 (18.79 vs 18.23 ms/step) and TP=4 (14.44 vs
-// 13.97): the ticket + reduce + 8-byte remote stores of the last split-K CTA of a tile lengthen the GEMM's tail by more
-// than the kernel boundary they save, because the publish kernel spreads the same work over 28 CTAs x 256 threads with
-// 16-byte stores (DESIGN.md §5, profiles/r02_tp_fused_publish_ab.md).
+// SSDK_FUSED_PUBLISH=1: the row-parallel GEMM publishes from its own epilogue (EPI_PUBLISH).  Off by default: the ticket +
+// reduce + 8-byte remote stores of the last split-K CTA of a tile lengthen the GEMM's tail, while the publish kernel
+// spreads the same work over 28 CTAs x 256 threads with 16-byte stores (DESIGN.md §5).
 static bool fused_publish_enabled() {
   static int v = -1;
   if (v < 0) {
@@ -881,7 +879,7 @@ static bool draft_stream_supported(const Model& m, int B) {
 }
 // Which draft path a step takes.  The streaming kernel wins while the attention phase of a KV split is ONE round of loads
 // (16 splits x 8 warps x 8 tokens = 1024 tokens); every further round costs more than the kernel-per-op draft's tensor-core
-// attention (measured at ~3k tokens: +2.4 ms per step, profiles/r02_draft_stream.md), so longer contexts take the
+// attention, so longer contexts take the
 // kernel-per-op graph.  Both graphs compute the same step; ctx_bound = the longest context of the batch before the step.
 static int draft_stream_max_ctx() {
   static int v = -1;

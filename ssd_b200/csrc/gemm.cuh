@@ -1,4 +1,4 @@
-// gemm.cuh — weight-streaming small-M GEMM on tcgen05 tensor cores (sm_100a).
+// gemm.cuh — weight-streaming small-M GEMM on Hopper warpgroup MMA (wgmma, sm_90a).
 //
 //   Y[M, N] = X[M, K] · W[N, K]^T        M <= 64 tokens, bf16 in, fp32 accumulate, bf16 out
 //
@@ -6,16 +6,18 @@
 // (layers/linear.py:98,196; layers/embed_head.py:95,111).  With M <= 7 the op is a pure
 // HBM stream of W (arithmetic intensity ~M flop/B), so the design goal is bytes in
 // flight, not tensor throughput:
-//   * swap-AB: the 128 weight rows of a tile are the UMMA "M" dimension, the (padded)
-//     tokens are the UMMA "N" dimension (16/32/64), so one tcgen05.mma consumes a
-//     128x16 (x bf16) weight slab whatever M is; the accumulator D[128 x UMMA_N] fp32
-//     lives in TMEM (32/64 columns).
+//   * swap-AB: the 128 weight rows of a tile are the MMA "M" dimension (two warpgroups x
+//     m64), the (padded) tokens are the MMA "N" dimension (16/32/64, 64-column chunks
+//     beyond), so one wgmma consumes a 64x16 (x bf16) weight slab whatever M is; the
+//     fp32 accumulator lives in the consumer warpgroups' registers.
 //   * W and X tiles arrive by TMA (cp.async.bulk.tensor.2d) into 128B-swizzled shared
 //     memory, kStages deep, mbarrier full/empty ring; W is tagged evict-first (read
 //     once per forward), X evict-last (re-read by every CTA from L2).
-//   * warp-specialised: warp 0 = TMA producer (one lane), warp 1 = TMEM allocator +
-//     MMA issuer (one lane), warps 2-5 = epilogue (tcgen05.ld -> registers -> global).
-//   * split-K over blockIdx.y fills the 148 SMs when N/128 is small; partial sums go to
+//   * warp-specialised: warps 0-3 / 4-7 = consumer warpgroups (wgmma on weight rows
+//     0-63 / 64-127), warp 8 = TMA producer (one lane).  The accumulator is staged through
+//     the (then idle) pipeline shared memory so that warpgroup 0 runs the epilogue with
+//     one weight row per thread.
+//   * split-K over blockIdx.y fills the SMs when N/128 is small; partial sums go to
 //     an fp32 [S, M, N] buffer which the *consumer* kernel (norm / rope / silu) reduces
 //     in a fixed order, so results are deterministic.
 //   * epilogues: bf16 store, fp32 split-K partial, or fused SiLU(gate)*up where a tile is
@@ -29,8 +31,9 @@
 namespace ssdk {
 
 constexpr int kBlockK = 64;    // bf16 per k-block = 128 B = one swizzle row
-constexpr int kTileRows = 128; // weight rows per CTA = UMMA_M
-constexpr int kGemmThreads = 192;
+constexpr int kTileRows = 128; // weight rows per CTA = 2 x wgmma M (64)
+constexpr int kGemmConsumers = 256;                // two consumer warpgroups
+constexpr int kGemmThreads = kGemmConsumers + 32;  // + the TMA producer warp
 
 enum GemmEpi { EPI_BF16 = 0, EPI_PARTIAL = 1, EPI_SILU = 2, EPI_PUBLISH = 3 };
 
@@ -67,7 +70,7 @@ struct GemmParams {
   PublishParams pub;      // EPI_PUBLISH only
 };
 
-// Split-K ticket reduction run by the 4 epilogue warps (threads 64..191).  `col` = this thread's column in the partial
+// Split-K ticket reduction run by the 4 epilogue warps (threads 0..127).  `col` = this thread's column in the partial
 // buffer (< 0: no column).  Returns true in the CTA that arrived last, with r[m] replaced by the sum over all splits.
 template <int UMMA_N>
 SSDK_DEVINL bool splitk_ticket_reduce(uint32_t* r, const GemmParams& p, int col, int tile, int* smem_flag) {
@@ -82,10 +85,10 @@ SSDK_DEVINL bool splitk_ticket_reduce(uint32_t* r, const GemmParams& p, int col,
   // the partial stores of the 128 epilogue threads are ordered before thread 64's acq_rel ticket by the named barrier
   // (one MEMBAR on one thread instead of a __threadfence on all of them); the same atomic is the acquire for the last CTA
   asm volatile("bar.sync 1, 128;" ::: "memory");
-  if (threadIdx.x == 64) *smem_flag = (atom_add_acq_rel_gpu(&p.sk_counters[tile], 1u) == (unsigned)S - 1u) ? 1 : 0;
+  if (threadIdx.x == 0) *smem_flag = (atom_add_acq_rel_gpu(&p.sk_counters[tile], 1u) == (unsigned)S - 1u) ? 1 : 0;
   asm volatile("bar.sync 1, 128;" ::: "memory");
   if (*smem_flag == 0) return false;
-  if (threadIdx.x == 64) st_relaxed_gpu_u32(&p.sk_counters[tile], 0u);  // every CTA of this tile has taken its ticket
+  if (threadIdx.x == 0) st_relaxed_gpu_u32(&p.sk_counters[tile], 0u);  // every CTA of this tile has taken its ticket
   if (col >= 0) {
     const size_t stride = (size_t)p.M * p.sk_width;
 #pragma unroll
@@ -114,11 +117,15 @@ struct GemmCfg {
   static constexpr int kStageBytes = kABytes + kBBytes;
   static constexpr int kStages = (UMMA_N == 16) ? 6 : (UMMA_N == 32 ? 5 : 4);
   static constexpr int kSmemBytes = kStages * kStageBytes + 1024;  // + alignment slack
-  static constexpr int kTmemCols = (UMMA_N <= 32) ? 32 : UMMA_N;   // power of two >= 32
   // UMMA_N <= 64 (decode / verify: weight streaming, two CTAs per SM keep ~190 KB of loads in flight); 128 / 256 (prefill
   // chunks and large batches: 128-192 KB of stages, one CTA per SM, the weights are read once per 128 / 256 tokens)
   static constexpr int kCtasPerSm = UMMA_N <= 64 ? 2 : 1;
   static constexpr int kEpiCols = UMMA_N < 64 ? UMMA_N : 64;       // accumulator columns handled per epilogue pass
+  static constexpr int kPasses = UMMA_N / kEpiCols;                // = wgmma N-chunks per k-step
+  // epilogue shared memory, carved from the drained pipeline: accumulator stage [128][kEpiCols + 1] fp32, then the
+  // SiLU exchange of the same size
+  static constexpr int kEpiBytes = kTileRows * (kEpiCols + 1) * 4;
+  static_assert(2 * kEpiBytes <= kStages * kStageBytes, "epilogue staging must fit in the pipeline stages");
 };
 
 template <int UMMA_N, int EPI>
@@ -126,12 +133,11 @@ __global__ void __launch_bounds__(kGemmThreads, GemmCfg<UMMA_N>::kCtasPerSm)
 gemm_ws_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmX, GemmParams p) {
   using Cfg = GemmCfg<UMMA_N>;
   constexpr int kStages = Cfg::kStages;
+  constexpr int CW = Cfg::kEpiCols;
 
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full_bar[kStages];
   __shared__ __align__(8) uint64_t empty_bar[kStages];
-  __shared__ __align__(8) uint64_t tmem_full_bar;
-  __shared__ uint32_t tmem_slot;
   __shared__ int pub_last;
 
   // 128B swizzle needs 1024 B aligned tiles
@@ -146,30 +152,22 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ 
   const int row_lo = (EPI == EPI_SILU) ? tile * 64 : tile * kTileRows;
   const int row_hi = row_lo + p.hi_row_offset;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == kGemmConsumers) {
     tma_prefetch_desc(&tmW);
     tma_prefetch_desc(&tmX);
 #pragma unroll
     for (int s = 0; s < kStages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], kGemmConsumers / 32);  // one arrival per consumer warp
     }
-    mbar_init(&tmem_full_bar, 1);
     fence_mbar_init();
   }
-  if (warp == 1) {
-    tmem_alloc(&tmem_slot, Cfg::kTmemCols);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_d = tmem_slot;
 
   // let the next kernel in the stream start its own prologue / weight prefetch
   pdl_launch_dependents();
 
-  if (warp == 0) {
+  if (threadIdx.x >= kGemmConsumers) {
     // ===================== TMA producer =====================
     if (lane == 0) {
       const int pre = min(nkb, kStages);
@@ -199,42 +197,62 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ 
         tma_load_2d(a_s + Cfg::kABytes, &tmX, &full_bar[s], k, 0, kEvictLast);
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_umma_idesc_bf16(kTileRows, UMMA_N);
-      for (int i = 0; i < nkb; ++i) {
-        const int s = i % kStages;
-        const uint32_t ph = (uint32_t)(i / kStages) & 1u;
-        mbar_wait(&full_bar[s], ph);
-        tc_fence_after();
-        uint8_t* a_s = smem + s * Cfg::kStageBytes;
-        const uint64_t adesc = make_umma_desc_k128(a_s);
-        const uint64_t bdesc = make_umma_desc_k128(a_s + Cfg::kABytes);
-#pragma unroll
-        for (int k = 0; k < kBlockK / 16; ++k) {
-          // advance 16 bf16 = 32 B along K inside the 128 B swizzle row: +2 in 16 B units
-          umma_bf16_ss(tmem_d, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), idesc, (uint32_t)((i | k) != 0));
-        }
-        umma_commit(&empty_bar[s]);  // frees the smem stage once these MMAs retire
-      }
-      umma_commit(&tmem_full_bar);  // accumulator complete
-    }
   } else {
-    // ===================== epilogue warps (2..5) =====================
+    // ===================== consumer warpgroups: MMA, then epilogue =====================
+    const int wg = warp >> 2;  // weight rows 64 wg .. 64 wg + 63 of the tile
+    float acc[Cfg::kPasses][CW / 2];
+#pragma unroll
+    for (int c = 0; c < Cfg::kPasses; ++c)
+#pragma unroll
+      for (int j = 0; j < CW / 2; ++j) acc[c][j] = 0.f;
+    for (int i = 0; i < nkb; ++i) {
+      const int s = i % kStages;
+      const uint32_t ph = (uint32_t)(i / kStages) & 1u;
+      mbar_wait(&full_bar[s], ph);
+      uint8_t* a_s = smem + s * Cfg::kStageBytes;
+      const uint64_t adesc = make_wgmma_desc_k128(a_s + wg * (Cfg::kABytes / 2));
+      const uint64_t bdesc = make_wgmma_desc_k128(a_s + Cfg::kABytes);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < kBlockK / 16; ++k) {
+        // advance 16 bf16 = 32 B along K inside the 128 B swizzle row: +2 in 16 B units; the next 64-token chunk of X
+        // starts 64 rows x 128 B = 8 KB further on
+#pragma unroll
+        for (int c = 0; c < Cfg::kPasses; ++c)
+          wgmma_bf16_ss<CW>(acc[c], adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k + c * (CW * 128 / 16)), 1u);
+      }
+      wgmma_commit();
+      wgmma_wait_all();
+      if (lane == 0) mbar_arrive(&empty_bar[s]);  // frees the smem stage: this warp's MMAs have retired
+    }
+
     pdl_wait();
-    const int q = warp & 3;  // TMEM lane quarter this warp may access
-    const int row = q * 32 + lane;
-    mbar_wait(&tmem_full_bar, 0);
-    tc_fence_after();
-    if (threadIdx.x == 64) trace_fine(TRF_GEMM + 0);  // CTA 0's accumulator complete
-    constexpr int CW = Cfg::kEpiCols;
+    if (threadIdx.x == 0) trace_fine(TRF_GEMM + 0);  // CTA 0's accumulator complete
+    // every consumer warp is past its last MMA and every TMA load has landed: the stages are free for the epilogue
+    asm volatile("bar.sync 2, %0;" ::"n"(kGemmConsumers) : "memory");
+    float* stage = reinterpret_cast<float*>(smem);
+    constexpr int LD = CW + 1;
+    const int frag_row = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int frag_col = 2 * (lane & 3);
+    const int row = threadIdx.x;  // epilogue (warpgroup 0): one weight row per thread
+    bool stop = false;            // SiLU split-K: another CTA of this tile finishes it
     // the accumulator is drained in passes of CW token columns (one pass for UMMA_N <= 64); token index = m0 + m
-    for (int m0 = 0; m0 < UMMA_N && m0 < p.M; m0 += CW) {
+#pragma unroll
+    for (int c = 0; c < Cfg::kPasses; ++c) {
+    const int m0 = c * CW;
+    if (m0 >= p.M || stop) break;
+#pragma unroll
+    for (int j = 0; j < CW / 8; ++j)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        stage[(frag_row + 8 * h) * LD + 8 * j + frag_col] = acc[c][4 * j + 2 * h];
+        stage[(frag_row + 8 * h) * LD + 8 * j + frag_col + 1] = acc[c][4 * j + 2 * h + 1];
+      }
+    asm volatile("bar.sync 2, %0;" ::"n"(kGemmConsumers) : "memory");
+    if (threadIdx.x < kTileRows) {
     uint32_t r[CW];
 #pragma unroll
-    for (int c = 0; c < CW / 16; ++c) tmem_ld_32x32b_x16(tmem_d + ((uint32_t)(q * 32) << 16) + m0 + c * 16, r + c * 16);
-    tmem_ld_wait();
+    for (int m = 0; m < CW; ++m) r[m] = __float_as_uint(stage[row * LD + m]);
 
     if (EPI == EPI_BF16) {
       const int n = row_lo + row;
@@ -285,15 +303,14 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ 
         const int j = row & 63;
         const int ncol = row_lo + j;
         const int col = ncol < p.N ? (row < 64 ? ncol : p.N + ncol) : -1;
-        if (!splitk_ticket_reduce<CW>(r, p, col, tile, &pub_last)) goto epilogue_done;
+        if (!splitk_ticket_reduce<CW>(r, p, col, tile, &pub_last)) goto epilogue_pass_done;
       }
-      // All MMAs have retired (tmem_full), so the pipeline stages are free to stage the exchange (128 x (CW + 1) floats).
-      float* ex = reinterpret_cast<float*>(smem);
-      constexpr int LD = CW + 1;
+      // the exchange (128 x (CW + 1) floats) sits behind the accumulator stage in the drained pipeline memory
+      float* ex = reinterpret_cast<float*>(smem + Cfg::kEpiBytes);
 #pragma unroll
       for (int m = 0; m < CW; ++m) ex[row * LD + m] = __uint_as_float(r[m]);
       asm volatile("bar.sync 1, 128;" ::: "memory");
-      const int e = threadIdx.x - 64;  // 0..127
+      const int e = threadIdx.x;  // 0..127
       __nv_bfloat16* out = reinterpret_cast<__nv_bfloat16*>(p.out);
       const int mc = min(CW, p.M - m0);
       for (int idx = e; idx < 64 * mc; idx += 128) {
@@ -307,16 +324,17 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ 
           out[(size_t)(m0 + m) * p.ldo + n] = f2bf(h);
         }
       }
-      if (UMMA_N > CW) asm volatile("bar.sync 1, 128;" ::: "memory");  // the next pass overwrites the exchange buffer
     }
+    }  // epilogue warpgroup
+  epilogue_pass_done:
+    // the next pass rewrites the stage; a SiLU split-K CTA that did not arrive last leaves the tile to the one that did
+    asm volatile("bar.sync 2, %0;" ::"n"(kGemmConsumers) : "memory");
+    stop = (EPI == EPI_SILU) && gridDim.y > 1 && pub_last == 0;
     }  // accumulator passes
   }
 
-epilogue_done:
-  tc_fence_before();
   __syncthreads();
-  if (threadIdx.x == 64) trace_fine(TRF_GEMM + 1);  // CTA 0's epilogue stored
-  if (warp == 1) tmem_dealloc(tmem_d, Cfg::kTmemCols);
+  if (threadIdx.x == 0) trace_fine(TRF_GEMM + 1);  // CTA 0's epilogue stored
 }
 
 // y[m, n] = bf16( sum_s P[s, m, n] )  — fixed-order split-K reduction (stand-alone op only;

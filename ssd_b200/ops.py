@@ -2,7 +2,7 @@
 reference's layers so the parity tests read like tests of ssd.layers.*).
 
 PyTorch is plumbing here: it owns the device memory and the stream; every op runs in the
-hand-written sm_100a kernels behind the C-ABI.  All functions require CUDA tensors and raise if
+hand-written sm_90a kernels behind the C-ABI.  All functions require CUDA tensors and raise if
 the extension is missing — there is no eager fallback.
 """
 from __future__ import annotations

@@ -1,4 +1,4 @@
-"""Tensor parallelism of the target across up to 8 B200s — one process per GPU.
+"""Tensor parallelism of the target across up to 8 GPUs — one process per GPU.
 
 The reference spawns one ModelRunner process per TP rank and drives them from rank 0 through pickle-over-shm RPC
 (engine/llm_engine.py:61-76, engine/model_runner.py:404-428).  Here every rank runs the SAME deterministic host

@@ -4,7 +4,7 @@ Unlike the reference, a missing SSD_HF_CACHE / SSD_DATASET_DIR does not raise at
 model directories (ssd_b200.synth) make the engine usable without any downloaded checkpoint."""
 import os
 
-CUDA_ARCH = os.environ.get("SSD_CUDA_ARCH", "10.0")  # B200; the reference defaults to 9.0 (paths.py:5)
+CUDA_ARCH = os.environ.get("SSD_CUDA_ARCH", "9.0")  # H100, as the reference (paths.py:5)
 HF_CACHE_DIR = os.environ.get("SSD_HF_CACHE", "/tmp/ssd_b200_models")
 DATASET_DIR = os.environ.get("SSD_DATASET_DIR", "/tmp/ssd_b200_datasets")
 

@@ -182,7 +182,7 @@ class PairRunner:
     def prefill(self, which: int, tokens: list[int], block_table: list[int], start: int = 0, temp: float = 0.0,
                 want_sample: bool = True, chunk: int = 256, seed: int = 0):
         """Prefill one sequence from position `start` in chunks of <= 256 tokens through the multi-query path: the
-        weights are streamed once per chunk (UMMA N = 128 / 256 instances of the tcgen05 GEMM), attention is the paged
+        weights are streamed once per chunk (UMMA N = 128 / 256 instances of the wgmma GEMM), attention is the paged
         multi-query kernel with one q tile per 4-32 query rows (layers/attention.py:85-93 semantics: causal over the
         cache, which already holds the earlier chunks)."""
         tok = None

@@ -19,6 +19,11 @@ def load(name: str):
 
 
 def trace_weights(z, prefix: str) -> dict:
+    """Weights of the traced target ("t") or draft ("d").  The draft is the target's embedding, head, final norm and
+    first layer, so only the target's weights are stored."""
+    if prefix == "d":
+        t = trace_weights(z, "t")
+        return {**t, "layers": t["layers"][:1]}
     w = {k: bf16(z[f"{prefix}_{k}"]) for k in ("embed", "lm_head", "final_norm")}
     layers = []
     l = 0

@@ -11,14 +11,15 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 def test_bytes_per_step_matches_baseline_md():
     sys.path.insert(0, ROOT)
     import bench
-    peak = 6571.2e9
-    rows = {("llama-3.1-8b", 1): 4.94, ("llama-3.1-70b", 1): 23.82, ("llama-3.1-70b", 2): 13.23, ("llama-3.1-70b", 4): 7.94,
-            ("llama-3.1-70b", 8): 5.29}
+    peak = 3350e9
+    rows = {("llama-3.1-8b", 1): 9.69, ("llama-3.1-70b", 1): 46.72, ("llama-3.1-70b", 2): 25.96, ("llama-3.1-70b", 4): 15.58,
+            ("llama-3.1-70b", 8): 10.38}
     for (t, tp), ms in rows.items():
         got = bench.bytes_per_step(t, "llama-3.2-1b", 6, 384, tp) / peak * 1e3
         assert abs(got - ms) < 0.02, (t, tp, got, ms)
-    q = bench.bytes_per_step("qwen3-32b", "qwen3-0.6b", 6, 384, 4) / peak * 1e3
-    assert abs(q - 3.75) < 0.02
+    for tp, ms in ((1, 21.71), (4, 7.37)):
+        q = bench.bytes_per_step("qwen3-32b", "qwen3-0.6b", 6, 384, tp) / peak * 1e3
+        assert abs(q - ms) < 0.02, (tp, q, ms)
 
 
 def test_reference_arm_prints_contract_keys():

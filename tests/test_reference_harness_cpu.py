@@ -1,21 +1,21 @@
-"""The reference's OWN acceptance harness (bench/bench.py, unmodified, SURVEY §2 item 19) driven on top of the
-ssd_b200 host engine through the `ssd` compat shim — on CPU, with the device runner replaced by a deterministic test
-double.  Checks the drop-in boundary end to end: `import ssd.paths`, `from ssd import LLM, SamplingParams`,
-`from ssd.engine.llm_engine import METRICS`, the kwargs of `create_llm_kwargs`, `generate()`'s return value, the sweep
-path that pokes `llm.config.max_num_seqs` / `llm.scheduler.max_num_seqs`, and the scheduler / block-manager bookkeeping
-under random accept lengths.  Skipped where the reference checkout is absent (the GPU box)."""
+"""The reference's OWN acceptance harness (bench/bench.py, unmodified, SURVEY §2 item 19) driving the ssd_b200 host
+engine through the `ssd` compat shim — on CPU, with the device runner replaced by a deterministic test double.
+
+The harness's calls into the engine were recorded by running it unmodified (oracle/gen_harness_golden.py ->
+tests/golden/harness_<case>.json): the model path and kwargs of its `create_llm_kwargs` -> `LLM(...)`, and per
+`generate()` the prompts, SamplingParams, the `llm.config.max_num_seqs` / `llm.scheduler.max_num_seqs` its sweep path
+sets and the METRICS it resets.  The tests replay those calls, in order, through `import ssd.paths`,
+`from ssd import LLM, SamplingParams` and `from ssd.engine.llm_engine import METRICS`, and check the drop-in boundary
+end to end: the configuration the kwargs produce, `generate()`'s return value, the sweep reconfiguration, and the
+scheduler / block-manager bookkeeping under random accept lengths."""
 import importlib
 import json
 import os
-import runpy
-import sys
 import types
 
 import numpy as np
-import pytest
 
-REF = "/root/reference"
-pytestmark = pytest.mark.skipif(not os.path.isdir(os.path.join(REF, "bench")), reason="reference checkout not present")
+from tests.helpers import GOLDEN
 
 V = 128256
 
@@ -82,7 +82,11 @@ def _make_hf_cache(root):
         os.rename(made, os.path.join(snap, "synthetic"))
 
 
-def _run_bench(tmp_path, monkeypatch, argv):
+def _run_bench(tmp_path, monkeypatch, case):
+    """Replay the reference harness's recorded calls (tests/golden/harness_<case>.json) on the engine."""
+    with open(GOLDEN / f"harness_{case}.json") as f:
+        rec = json.load(f)
+    assert rec["exit_code"] == 0
     monkeypatch.setenv("SSD_HF_CACHE", str(tmp_path))
     monkeypatch.setenv("SSD_DATASET_DIR", str(tmp_path / "datasets"))
     _make_hf_cache(str(tmp_path))
@@ -90,9 +94,6 @@ def _run_bench(tmp_path, monkeypatch, argv):
     importlib.reload(P)
     import ssd_b200.compat as compat
     compat.install()
-    wandb = types.ModuleType("wandb")
-    wandb.init = wandb.log = wandb.finish = lambda *a, **k: None
-    monkeypatch.setitem(sys.modules, "wandb", wandb)
     fake = {}
 
     def fake_build_runner(config, tp_size=1, tp_rank=0, device=None, finalize=True):
@@ -103,27 +104,32 @@ def _run_bench(tmp_path, monkeypatch, argv):
 
     import ssd_b200.loader as loader
     monkeypatch.setattr(loader, "build_runner", fake_build_runner)
+
+    import ssd.paths  # noqa: F401  (the harness's first import)
+    from ssd import LLM, SamplingParams
+    from ssd.engine.llm_engine import METRICS
+    path = lambda v: v.replace("{HF_CACHE}", str(tmp_path)) if isinstance(v, str) else v
+    llm = LLM(path(rec["llm"]["model"]), **{k: path(v) for k, v in rec["llm"]["kwargs"].items()})
     captured = {}
-    import ssd_b200.engine.llm_engine as eng
-    orig_generate = eng.LLMEngine.generate
-
-    def spy_generate(self, prompts, sampling_params, use_tqdm=True, stream_callback=None):
-        outs, metrics = orig_generate(self, prompts, sampling_params, use_tqdm=False, stream_callback=stream_callback)
+    for run in rec["runs"]:
+        b = run["config_max_num_seqs"]
+        assert b <= llm.config.max_num_seqs  # the harness's reconfigure_engine contract
+        llm.config.max_num_seqs = b
+        llm.scheduler.max_num_seqs = run["scheduler_max_num_seqs"]
+        for k, v in METRICS.items():  # the harness's reset_metrics
+            if isinstance(v, list):
+                v.clear()
+            else:
+                METRICS[k] = 0
+        assert {k: (list(v) if isinstance(v, list) else v) for k, v in METRICS.items()} == run["metrics_at_call"]
+        prompts = run["prompts"]
+        outs, metrics = llm.generate(prompts, [SamplingParams(**sp) for sp in run["sampling_params"]], use_tqdm=False)
         captured.setdefault("runs", []).append((prompts, outs, {k: (list(v) if isinstance(v, list) else v) for k, v in metrics.items()}))
-        return outs, metrics
-
-    monkeypatch.setattr(eng.LLMEngine, "generate", spy_generate)
-    monkeypatch.setattr(sys, "argv", ["bench.py"] + argv)
-    monkeypatch.syspath_prepend(os.path.join(REF, "bench"))
-    with pytest.raises(SystemExit) as ex:
-        runpy.run_path(os.path.join(REF, "bench", "bench.py"), run_name="__main__")
-    assert ex.value.code == 0
     return captured, fake
 
 
 def test_reference_bench_py_runs_unmodified_on_the_engine(tmp_path, monkeypatch):
-    captured, fake = _run_bench(tmp_path, monkeypatch, ["--size", "8", "--spec", "--k", "6", "--random", "--numseqs", "5",
-                                                       "--input_len", "40", "--output_len", "60", "--b", "2"])
+    captured, fake = _run_bench(tmp_path, monkeypatch, "spec")
     cfg = fake["config"]
     assert cfg.speculate and cfg.speculate_k == 6 and cfg.jit_speculate and cfg.kvcache_block_size == 256
     assert cfg.max_num_seqs == 2 and cfg.max_model_len == 8192
@@ -144,9 +150,7 @@ def test_reference_bench_py_runs_unmodified_on_the_engine(tmp_path, monkeypatch)
 
 
 def test_reference_bench_py_sweep_and_autoregressive(tmp_path, monkeypatch):
-    captured, fake = _run_bench(tmp_path, monkeypatch, ["--size", "8", "--random", "--numseqs", "3", "--input_len", "16",
-                                                       "--output_len", "20", "--b", "2",
-                                                       "--sweep", json.dumps([{"b": 2, "temp": 0.5}, {"b": 1}])])
+    captured, fake = _run_bench(tmp_path, monkeypatch, "sweep_ar")
     assert not fake["config"].speculate
     assert len(captured["runs"]) == 2
     for prompts, outs, metrics in captured["runs"]:

@@ -1,7 +1,7 @@
 """Tensor-parallel hot path on 2 GPUs (one process per GPU, NCCL): prefill + speculative steps through the C-ABI on
 both ranks, rank 0's verdicts checked against the single-device CPU oracle (teacher-forced, near-tie protocol).
 Covers the in-graph collectives: embedding all-reduce, row-parallel all-reduce, vocab-parallel lm_head all-gather,
-draft-token broadcast, verdict broadcast.  Needs >= 2 GPUs (gpurun --gpus 2)."""
+draft-token broadcast, verdict broadcast.  Needs >= 2 GPUs; skips on one."""
 import socket
 
 import pytest

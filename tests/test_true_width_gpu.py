@@ -10,8 +10,7 @@ the C-ABI (ssdk_forward_tokens / ssdk_spec_step):
   * logits_p / logits_q at 2048 sampled vocabulary columns of every row: |diff| <= 2.5 + 2^-5 |ref| everywhere AND a mean
     |diff| <= 0.6.  Calibration of these bounds (bf16 logits of magnitude 70-90, spacing 0.5): the oracle's OWN two
     arithmetic variants — Inductor single-rounding vs eager double-rounding norms / SiLU, oracle/ops.py `compiled` —
-    differ from each other by mean 0.127 / max 1.0 (8B widths) and mean 0.348 / max 2.0 (70B widths); this engine against
-    the oracle measures mean 0.138 (8B), 0.178 (Qwen3-32B), 0.376 / max 1.7 (70B) on B200: the same one-ulp noise.  A real
+    differ from each other by mean 0.127 / max 1.0 (8B widths) and mean 0.348 / max 2.0 (70B widths): one-ulp noise.  A real
     defect is far outside: switching the attention branch or the MLP branch off moves the target's sampled logits by 9 on
     average (max 64), the 1B-width draft's by 2 on average;
   * the top-1 logit of every row within 2^-6 relative.

@@ -1,5 +1,5 @@
 """Stand-alone timing of ssdk_paged_attn (attention + split-KV combine) at the shapes of the speculative step, next to
-flash_attn 2.8.3's `flash_attn_with_kvcache` (the sm_100-enabled library kernel the reference GPU arm runs behind its
+flash_attn 2.8.3's `flash_attn_with_kvcache` (the library kernel the reference GPU arm runs behind its
 sgl_kernel stub) on the SAME paged cache, for context 135 ... 8192.  Launches are captured in a CUDA graph (100 per replay)
 so the number is the kernel time without host launch gaps; warm-L2 figure (as in the step, where the new tokens' K/V were
 just written).  Also prints the achieved KV bytes/s of ours: ctx * KV * hd * 2 (K and V) * 2 B per launch."""

@@ -1,5 +1,6 @@
 """Micro-benchmark of the weight-streaming GEMM at the shapes of the BASELINE models: achieved HBM GB/s
-(weight bytes / CUDA-event time, L2 flushed between launches) next to torch (cuBLAS) on the same shapes."""
+(weight bytes / CUDA-event time, L2 flushed between launches) next to torch (cuBLAS) on the same shapes.
+    python tools/bench_gemm.py [OUT.json]"""
 import json
 import os
 import sys
@@ -49,7 +50,9 @@ def main():
             print(json.dumps(rec), flush=True)
             out.append(rec)
         del w
-    json.dump(out, open("gpurun_out/gemm_bench.json", "w"), indent=1)
+    if len(sys.argv) > 1:  # optional file for the records printed above
+        with open(sys.argv[1], "w") as f:
+            json.dump(out, f, indent=1)
 
 
 if __name__ == "__main__":

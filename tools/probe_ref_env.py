@@ -1,4 +1,4 @@
-"""GPU-box probe: do flash_attn 2.8.3 (paged kvcache, sm_100) and torch.compile (Inductor -> Triton) work here?
+"""GPU probe: do flash_attn 2.8.3 (paged kvcache) and torch.compile (Inductor -> Triton) work here?
 Both are prerequisites of the reference GPU arm (bench.py --impl reference-gpu)."""
 import time
 import torch

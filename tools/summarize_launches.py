@@ -1,4 +1,4 @@
-"""Summarise an `ncu --metrics gpu__time_duration.sum --csv` launch list into a markdown table (profiles/)."""
+"""Summarise an `ncu --metrics gpu__time_duration.sum --csv` launch list into a markdown table."""
 import collections
 import csv
 import re

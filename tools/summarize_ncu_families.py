@@ -1,6 +1,6 @@
-"""gpurun_out/ncu/r02_*.raw.csv (ncu --set full, `--page raw --csv`, tools/gpu_ncu_families.sh) -> one markdown table.
+"""<dir>/*.raw.csv (ncu --set full, `--page raw --csv`, one capture per kernel family) -> one markdown table.
 
-    python tools/summarize_ncu_families.py gpurun_out/ncu > profiles/r02_ncu_families.md
+    python tools/summarize_ncu_families.py <ncu report dir> > ncu_families.md
 
 One row per captured launch: grid, registers, duration, DRAM bytes read / written, achieved DRAM GB/s and its fraction of
 the measured HBM peak (MEASURED_PEAKS.json), ncu's DRAM- and SM-throughput percentages and the L2 hit rate."""
@@ -25,7 +25,7 @@ def to_us(v: str, unit: str) -> float:
 
 
 def main():
-    d = sys.argv[1] if len(sys.argv) > 1 else os.path.join(ROOT, "gpurun_out", "ncu")
+    d = sys.argv[1]
     peak = 6571.2
     try:
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
@@ -35,7 +35,7 @@ def main():
     print("| capture | kernel | grid x block | regs | duration (us) | dram read | dram written | DRAM GB/s | of measured peak "
           f"({peak:.1f}) | dram % | sm % | L2 hit % |")
     print("|---|---|---|---:|---:|---:|---:|---:|---:|---:|---:|---:|")
-    for path in sorted(glob.glob(os.path.join(d, "r02_*.raw.csv"))):
+    for path in sorted(glob.glob(os.path.join(d, "*.raw.csv"))):
         cap = os.path.basename(path)[4:-8]
         rows = list(csv.reader(open(path)))
         if len(rows) < 3:
