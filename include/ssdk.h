@@ -235,6 +235,10 @@ int ssdk_paged_attn(const void* q, const void* k_cache, const void* v_cache,
                     void* out, void* scratch,
                     int batch, int q_len, int heads, int kv_heads, int head_dim,
                     int block_size, int max_blocks_per_seq, float scale, void* stream);
+/* The launch plan ssdk_paged_attn picks for these sizes on the current device (max_ctx = block_size *
+ * max_blocks_per_seq): out4 = {TQ query tokens per tile, MT 16-row MMA tiles per tile, n_qtiles, n_split KV splits}.
+ * Launches nothing. */
+int ssdk_paged_attn_plan(int heads, int kv_heads, int batch, int q_len, int max_ctx, int* out4);
 
 /* Sampler.forward (layers/sampler.py:14-36): greedy where temp==0, else
  * argmax(softmax(l/T) / Exp(1)) with Philox(seed, step_id) exponentials.

@@ -1,5 +1,5 @@
 // attention.cuh — paged attention for decode (q_len = 1), verify (q_len = K+1) and
-// prefill chunks (q_len <= 64) over the 256-token-page KV cache.
+// prefill chunks (q_len <= 256) over the paged KV cache (any page size; 256 tokens in the reference).
 // Replaces sgl_kernel.flash_attn.flash_attn_with_kvcache at layers/attention.py:107-111,128-131:
 //   softmax(q k^T * hd^-1/2 + causal) v, GQA (query head h -> kv head h / (H/KV)),
 //   causal mask aligned to the END of the cache (query j of a sequence sees kv positions
@@ -27,6 +27,45 @@ namespace ssdk {
 // generation, softmax, epilogue merge) rather than by bandwidth: more warps = shorter chains.
 constexpr int attn_warps(int MT) { return MT == 1 ? 4 : 8; }
 constexpr int kAttChunk = 64;
+constexpr int kAttnMaxSplit = 32;  // split-KV partials per (token, head) row; attn_combine_kernel merges up to 32
+
+// Launch plan (host code, shared by the engine and the host-thread test driver).
+struct AttnPlan {
+  int TQ;        // query tokens per CTA tile
+  int MT;        // 16-row MMA tiles per CTA (G * TQ rows, padded)
+  int n_qtiles;  // ceil(Q / TQ)
+  int n_split;   // KV splits per (kv head, sequence, q tile)
+};
+// q tile of <= 32 rows (two 16-row MMA tiles, 8 warps = 4 token slices each): faster per verify layer than one 56-row
+// tile or 16-row tiles.  KV is split until there are about two CTAs per SM, at most kAttnMaxSplit ways and at most one
+// split per 64-token chunk of max_ctx.  Returns 1 for an unsupported GQA ratio, 2 for a tile that is too large.
+inline int attn_make_plan(int H, int KV, int B, int Q, int max_ctx, int n_sms, AttnPlan* pl) {
+  if (KV < 1) return 1;
+  const int G = H / KV;
+  if (G < 1|| G > 16 || (H % KV) != 0) return 1;
+  int tq = 32 / G;
+  if (tq < 1) tq = 1;
+  if (tq > Q) tq = Q;
+  int mt = (G * tq + 15) / 16;
+  if (mt == 3) mt = 4;
+  if (mt > 4) return 2;
+  pl->TQ = tq;
+  pl->MT = mt;
+  pl->n_qtiles = (Q + tq - 1) / tq;
+  const int ctas = KV * B * pl->n_qtiles;
+  int ns = (2 * n_sms + ctas - 1) / ctas;
+  const int max_chunks = max_ctx > kAttChunk ? (max_ctx + kAttChunk - 1) / kAttChunk : 1;
+  if (ns > kAttnMaxSplit) ns = kAttnMaxSplit;
+  if (ns > max_chunks) ns = max_chunks;
+  pl->n_split = ns < 1 ? 1 : ns;
+  return 0;
+}
+// AttnParams::g_shift
+inline int attn_g_shift(int H, int KV) {
+  for (int sft = 0; sft < 5; ++sft)
+    if (H / KV == (1 << sft)) return sft;
+  return -1;
+}
 
 struct AttnParams {
   const __nv_bfloat16* q;        // [B*Q, H, hd]
@@ -42,6 +81,8 @@ struct AttnParams {
   float scale_log2;              // softmax scale * log2(e)
 };
 
+#ifndef SSDK_HOST_EMU
+// tests/emu/cuda_emu.h supplies host stand-ins for these five
 SSDK_DEVINL void cp_async16(void* smem_dst, const void* gsrc, bool valid) {
   const int sz = valid ? 16 : 0;
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(smem_dst)), "l"(gsrc), "r"(sz)
@@ -69,6 +110,7 @@ SSDK_DEVINL void mma_bf16_16816(float* c, const uint32_t* a, uint32_t b0, uint32
       : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
+#endif
 SSDK_DEVINL uint32_t pack_bf16x2(float lo, float hi) {
   __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
   return *reinterpret_cast<uint32_t*>(&v);
@@ -86,7 +128,7 @@ __global__ void __launch_bounds__(attn_warps(MT) * 32) paged_attn_kernel(AttnPar
   constexpr int ND = HD / 8;                // 8-wide output tiles over head_dim
   constexpr int SEG = HD / 8;               // 16-byte segments per K/V row
 
-  extern __shared__ __align__(16) uint8_t att_smem[];
+  SSDK_DYN_SMEM(uint8_t, att_smem);
   __nv_bfloat16* sK = reinterpret_cast<__nv_bfloat16*>(att_smem);            // [2][64][LDS]
   __nv_bfloat16* sV = sK + 2 * kAttChunk * LDS;                              // [2][64][LDS]
 
@@ -348,7 +390,7 @@ __global__ void __launch_bounds__(attn_warps(MT) * 32) paged_attn_kernel(AttnPar
 // chunks (n_active, recomputed from context_lens with the attention kernel's formula) are read, and every thread
 // issues all of its loads before using them, so the merge costs ~2 L2 round trips whatever n_split is.
 __global__ void attn_combine_kernel(AttnParams p, int hd) {
-  __shared__ float sw[32];
+  SSDK_STATIC_SMEM(float, sw, 32);
   pdl_launch_dependents();
   pdl_wait();
   if (threadIdx.x == 0) trace_mark(TR_ATTN);

@@ -1,7 +1,7 @@
 // common.cuh — shared device helpers for the sm_90a kernels of libssdk.
 // PTX wrappers (mbarrier, TMA, wgmma, PDL), bf16 helpers, reductions, Philox.
 #pragma once
-// SSDK_HOST_EMU: the kernels that use no tensor-core / TMA / PTX-only feature can be compiled for the host by the test
+// SSDK_HOST_EMU: the kernels that use no TMA / wgmma / PTX-only feature can be compiled for the host by the test
 // suite (tests/emu/cuda_emu.h supplies the CUDA vocabulary before this header is included); never defined in the product.
 #ifndef SSDK_HOST_EMU
 #include <cuda_runtime.h>

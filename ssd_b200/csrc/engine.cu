@@ -288,7 +288,6 @@ struct Workspace {
 constexpr int kSampleChunks = 64;
 constexpr int kLogCap = 16384;
 constexpr int kVerifyCtas = 128;
-constexpr int kAttnMaxSplit = 32;
 
 struct ssdk_engine {
   ssdk_runtime_cfg rt;
@@ -435,25 +434,19 @@ struct Fwd {
   int64_t logits_ld;
 };
 
-static int attn_plan(const Model& m, int B, int Q, int* TQ, int* MT, int* nqt, int* nsplit, int max_ctx) {
-  const int G = m.H / m.KV;
-  if (G < 1 || G > 16 || (m.H % m.KV) != 0) return fail("unsupported GQA ratio %d", G);
-  // q tile of <= 32 rows (two 16-row MMA tiles, 8 warps = 4 token slices each): faster per verify layer than one 56-row
-  // tile or 16-row tiles
-  int tq = std::min(Q, std::max(1, 32 / G));
-  int R = G * tq;
-  int mt = (R + 15) / 16;
-  if (mt == 3) mt = 4;
-  if (mt > 4) return fail("attention tile too large");
-  *TQ = tq;
-  *MT = mt;
-  *nqt = (Q + tq - 1) / tq;
-  const int ctas = m.KV * B * (*nqt);
-  int ns = (2 * num_sms() + ctas - 1) / ctas;
-  const int max_chunks = std::max(1, (max_ctx + kAttChunk - 1) / kAttChunk);
-  ns = std::max(1, std::min(std::min(ns, kAttnMaxSplit), max_chunks));
-  *nsplit = ns;
+static int attn_plan_raw(int H, int KV, int B, int Q, int max_ctx, int* TQ, int* MT, int* nqt, int* nsplit) {
+  AttnPlan pl;
+  const int rc = attn_make_plan(H, KV, B, Q, max_ctx, num_sms(), &pl);
+  if (rc == 1) return fail("unsupported GQA ratio %d/%d", H, KV);
+  if (rc != 0) return fail("attention tile too large");
+  *TQ = pl.TQ;
+  *MT = pl.MT;
+  *nqt = pl.n_qtiles;
+  *nsplit = pl.n_split;
   return 0;
+}
+static int attn_plan(const Model& m, int B, int Q, int* TQ, int* MT, int* nqt, int* nsplit, int max_ctx) {
+  return attn_plan_raw(m.H, m.KV, B, Q, max_ctx, TQ, MT, nqt, nsplit);
 }
 
 template <int HD, int MT>
@@ -487,9 +480,7 @@ static int enqueue_attention(Launcher& L, const bf16* q, const bf16* kc, const b
   (void)counters;
   a.B = B; a.Q = Q; a.H = H; a.KV = KV; a.block_size = block_size; a.max_blocks = max_blocks;
   a.n_split = nsplit; a.TQ = TQ; a.n_qtiles = nqt;
-  a.g_shift = -1;
-  for (int sft = 0; sft < 5; ++sft)
-    if ((H / KV) == (1 << sft)) a.g_shift = sft;
+  a.g_shift = attn_g_shift(H, KV);
   a.scale_log2 = scale * 1.4426950408889634f;
   CKI(launch_attn(L, a, hd, MT, dim3(KV, nsplit, B * nqt)));
   if (nsplit > 1) CKI(L.go(attn_combine_kernel, dim3(B * Q * H), dim3(32), 0, a, hd));
@@ -1585,11 +1576,9 @@ int ssdk_silu_mul(const void* gate_up, void* out, int M, int ffn, void* stream) 
   return L.go(silu_mul_kernel, dim3((M * ffn / 8 + 255) / 256), dim3(256), 0, g, (bf16*)out, M, ffn);
 }
 
-static int attn_plan_raw(int H, int KV, int B, int Q, int max_ctx, int* TQ, int* MT, int* nqt, int* nsplit) {
-  Model tmp;
-  tmp.H = H;
-  tmp.KV = KV;
-  return attn_plan(tmp, B, Q, TQ, MT, nqt, nsplit, max_ctx);
+int ssdk_paged_attn_plan(int heads, int kv_heads, int batch, int q_len, int max_ctx, int* out4) {
+  if (batch < 1 || q_len < 1 || kv_heads < 1 || out4 == nullptr) return fail("paged_attn_plan: bad arguments");
+  return attn_plan_raw(heads, kv_heads, batch, q_len, max_ctx, &out4[0], &out4[1], &out4[2], &out4[3]);
 }
 
 int64_t ssdk_paged_attn_scratch_bytes(int batch, int q_len, int heads, int head_dim, int max_ctx) {

@@ -79,6 +79,7 @@ SIGNATURES: dict[str, tuple] = {
     "ssdk_paged_attn_scratch_bytes": (C.c_int64, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
     "ssdk_paged_attn": (C.c_int, [VP, VP, VP, VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                   C.c_int, C.c_float, VP]),
+    "ssdk_paged_attn_plan": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, c_i32p]),
     "ssdk_sample": (C.c_int, [VP, C.c_int64, VP, C.c_int, C.c_int, C.c_uint64, C.c_uint64, VP, VP]),
     "ssdk_verify_scratch_bytes": (C.c_int64, [C.c_int, C.c_int]),
     "ssdk_verify": (C.c_int, [VP, VP, VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_uint64, C.c_uint64,

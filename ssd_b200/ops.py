@@ -7,6 +7,8 @@ the extension is missing — there is no eager fallback.
 """
 from __future__ import annotations
 
+import ctypes as C
+
 import torch
 
 from . import lib as _L
@@ -136,6 +138,15 @@ def paged_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tenso
                                  _ptr(scratch), B, q_len, H, KV, hd, block_size, max_blocks, float(scale), _stream()),
              "ssdk_paged_attn")
     return out
+
+
+def paged_attention_plan(B: int, q_len: int, H: int, KV: int, max_ctx: int) -> dict:
+    """The launch plan paged_attention takes for these sizes on the current device (max_ctx = block_size *
+    max_blocks): query tokens per tile, 16-row MMA tiles, query tiles and KV splits."""
+    out = (C.c_int32 * 4)()
+    lib = _L.load()
+    _L.check(lib.ssdk_paged_attn_plan(H, KV, B, q_len, max_ctx, out), "ssdk_paged_attn_plan")
+    return {"TQ": out[0], "MT": out[1], "n_qtiles": out[2], "n_split": out[3]}
 
 
 def sample(logits: torch.Tensor, temperatures: torch.Tensor, seed: int = 0, step_id: int = 0) -> torch.Tensor:

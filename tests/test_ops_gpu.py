@@ -4,6 +4,7 @@ import numpy as np
 import pytest
 import torch
 
+from tests import attn_ref
 from tests.helpers import bf16, load, ulp_mismatch_fraction
 
 pytestmark = pytest.mark.gpu
@@ -122,7 +123,6 @@ def test_rope_store_kv(dev, H, KV, hd, qk_norm):
 @pytest.mark.parametrize("q_len,ctx", [(1, [1]), (1, [63, 300]), (7, [7]), (7, [64, 65]), (5, [1000, 257]), (40, [40]),
                                        (64, [200]), (200, [200]), (256, [700]), (100, [100, 356])])
 def test_paged_attention(dev, H, KV, hd, q_len, ctx):
-    from oracle import ops as O
     from ssd_b200 import ops
     g = torch.Generator().manual_seed(H + KV + hd + q_len + sum(ctx))
     B, bs = len(ctx), 256
@@ -139,9 +139,12 @@ def test_paged_attention(dev, H, KV, hd, q_len, ctx):
         bt[b, used:] = -1
     q = torch.randn(B * q_len, H, hd, generator=g).to(torch.bfloat16)
     cl = torch.tensor(ctx, dtype=torch.int32)
-    ref = O.paged_attention(q, kc, vc, bt.clamp(min=0), cl, q_len, hd ** -0.5)
     out = ops.paged_attention(q.to(dev), kc.to(dev), vc.to(dev), bt.to(dev), cl.to(dev), q_len, hd ** -0.5).cpu()
-    torch.testing.assert_close(out.float(), ref.float(), rtol=3e-2, atol=2e-2)
+    # fp64 reference, within twice the kernel's two bf16 roundings (tests/attn_ref.py; test_attention_gpu.py has the
+    # needle inputs, page sizes, GQA ratios and split plans)
+    ref, S = attn_ref.reference(q, kc, vc, bt, cl, q_len, hd ** -0.5)
+    r = attn_ref.err_over_bound(out, ref, S)
+    assert r <= 1.0, f"worst err/bound {r:.3f}"
 
 
 def test_sample_greedy_and_ties(dev):
