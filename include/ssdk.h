@@ -72,7 +72,7 @@ typedef struct ssdk_model_cfg {
 
 typedef struct ssdk_runtime_cfg {
   int32_t spec_k;             /* K (speculate_k); 0 = autoregressive only */
-  int32_t max_batch;          /* max sequences per step (b); max_batch*(K+1) <= 64 */
+  int32_t max_batch;          /* max sequences per step (b); max_batch*(K+1) <= 256, max_batch <= 32 */
   int32_t block_size;         /* KV page size (kvcache_block_size, 256 in bench.py:40) */
   int32_t max_blocks_per_seq; /* ceil(max_model_len / block_size) */
   int32_t use_graph;          /* 1 = capture the spec step into one CUDA graph */
@@ -163,7 +163,7 @@ int ssdk_spec_step_fetch(ssdk_handle h, int batch, int64_t* out_tokens,
 int ssdk_spec_step_log(ssdk_handle h, int seq, int64_t* out_tokens, int cap, void* stream);
 
 /* Generic multi-token forward + sample of the last position of every sequence.
- * Replaces ModelRunner.run for prefill chunks (q_len<=64 per call, causal over the
+ * Replaces ModelRunner.run for prefill chunks (batch*q_len<=256 per call, causal over the
  * paged cache; engine/model_runner.py:634-680 with is_prefill) and for
  * single-token autoregressive decode (q_len=1; engine/step.py:36-47).
  *   ids[b*q_len + j] tokens, written to positions ctx_len[b]+j.
@@ -176,9 +176,22 @@ int ssdk_forward_tokens(ssdk_handle h, int which, int batch, int q_len,
                         const float* temps, uint64_t seed, uint64_t step_id,
                         int64_t* out_tokens, void* stream);
 
+/* ssdk_forward_tokens for sequences of different lengths in one call (the reference's
+ * cu_seqlens prefill, engine/helpers/runner_helpers.py:123-180): q_lens[b] tokens of
+ * sequence b, packed in sequence order in ids (sum of q_lens long), written to positions
+ * ctx_len[b] .. ctx_len[b]+q_lens[b]-1; ctx_len[b] tokens are already in the cache.
+ * 1 <= n_seqs <= max_batch, every q_lens[b] >= 1, sum <= 256.  want_sample: lm_head on the
+ * last row of every sequence, sampled into out_tokens[b]; ssdk_logits_last then holds
+ * [n_seqs, V].  Blocks until out_tokens is on the host when want_sample != 0. */
+int ssdk_forward_varlen(ssdk_handle h, int which, int n_seqs, const int32_t* q_lens,
+                        const int64_t* ids, const int32_t* ctx_len,
+                        const int32_t* block_tables, int want_sample,
+                        const float* temps, uint64_t seed, uint64_t step_id,
+                        int64_t* out_tokens, void* stream);
+
 /* Debug/parity taps: device pointers to the logits of the last spec step
  * (bf16 [batch, K+1, V] and [batch, K, V]) and of the last ssdk_forward_tokens
- * (bf16 [batch, V]).  Valid until the next call. */
+ * or ssdk_forward_varlen (bf16 [batch, V]).  Valid until the next call. */
 const void* ssdk_logits_p(ssdk_handle h);
 const void* ssdk_logits_q(ssdk_handle h);
 const void* ssdk_logits_last(ssdk_handle h);
@@ -239,6 +252,18 @@ int ssdk_paged_attn(const void* q, const void* k_cache, const void* v_cache,
  * max_blocks_per_seq): out4 = {TQ query tokens per tile, MT 16-row MMA tiles per tile, n_qtiles, n_split KV splits}.
  * Launches nothing. */
 int ssdk_paged_attn_plan(int heads, int kv_heads, int batch, int q_len, int max_ctx, int* out4);
+/* ssdk_paged_attn for `batch` sequences of their own q_lens[b] (host array), packed in sequence
+ * order: q [sum q_lens, H, hd] -> out [sum q_lens, H*hd]; context_lens[b] includes the q_lens[b]
+ * new tokens.  Query tiles never cross a sequence.  `scratch`: at least
+ * ssdk_paged_attn_scratch_bytes(1, sum q_lens, heads, head_dim, max_ctx) bytes. */
+int ssdk_paged_attn_varlen(const void* q, const void* k_cache, const void* v_cache,
+                           const int32_t* block_tables, const int32_t* context_lens,
+                           const int32_t* q_lens, void* out, void* scratch,
+                           int batch, int heads, int kv_heads, int head_dim,
+                           int block_size, int max_blocks_per_seq, float scale, void* stream);
+/* Its plan: out5 = {TQ, MT, n_qtiles of the longest sequence, n_split, tiles in the launch}.
+ * With every q_lens[b] equal the first four are ssdk_paged_attn_plan's. */
+int ssdk_paged_attn_varlen_plan(int heads, int kv_heads, int batch, const int32_t* q_lens, int max_ctx, int* out5);
 
 /* Sampler.forward (layers/sampler.py:14-36): greedy where temp==0, else
  * argmax(softmax(l/T) / Exp(1)) with Philox(seed, step_id) exponentials.

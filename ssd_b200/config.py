@@ -46,6 +46,9 @@ class Config:
     use_cuda_graph: bool = True
     use_pdl: bool = True
     seed: int = 0
+    # prefill through ssdk_forward_varlen (PairRunner.prefill_varlen): prompts of any lengths and prefix-cache hits share
+    # 256-token calls.  Opt-in until measured on the H100 (DESIGN.md §7).
+    varlen_prefill: bool = False
 
     @property
     def max_blocks(self) -> int:

@@ -37,9 +37,8 @@ struct AttnPlan {
   int n_split;   // KV splits per (kv head, sequence, q tile)
 };
 // q tile of <= 32 rows (two 16-row MMA tiles, 8 warps = 4 token slices each): faster per verify layer than one 56-row
-// tile or 16-row tiles.  KV is split until there are about two CTAs per SM, at most kAttnMaxSplit ways and at most one
-// split per 64-token chunk of max_ctx.  Returns 1 for an unsupported GQA ratio, 2 for a tile that is too large.
-inline int attn_make_plan(int H, int KV, int B, int Q, int max_ctx, int n_sms, AttnPlan* pl) {
+// tile or 16-row tiles.  Returns 1 for an unsupported GQA ratio, 2 for a tile that is too large.
+inline int attn_tile_shape(int H, int KV, int Q, AttnPlan* pl) {
   if (KV < 1) return 1;
   const int G = H / KV;
   if (G < 1|| G > 16 || (H % KV) != 0) return 1;
@@ -51,14 +50,69 @@ inline int attn_make_plan(int H, int KV, int B, int Q, int max_ctx, int n_sms, A
   if (mt > 4) return 2;
   pl->TQ = tq;
   pl->MT = mt;
-  pl->n_qtiles = (Q + tq - 1) / tq;
-  const int ctas = KV * B * pl->n_qtiles;
+  return 0;
+}
+// KV is split until there are about two CTAs per SM, at most kAttnMaxSplit ways and at most one split per 64-token
+// chunk of max_ctx.
+inline int attn_split_count(int ctas, int max_ctx, int n_sms) {
   int ns = (2 * n_sms + ctas - 1) / ctas;
   const int max_chunks = max_ctx > kAttChunk ? (max_ctx + kAttChunk - 1) / kAttChunk : 1;
   if (ns > kAttnMaxSplit) ns = kAttnMaxSplit;
   if (ns > max_chunks) ns = max_chunks;
-  pl->n_split = ns < 1 ? 1 : ns;
+  return ns < 1 ? 1 : ns;
+}
+inline int attn_make_plan(int H, int KV, int B, int Q, int max_ctx, int n_sms, AttnPlan* pl) {
+  const int rc = attn_tile_shape(H, KV, Q, pl);
+  if (rc != 0) return rc;
+  pl->n_qtiles = (Q + pl->TQ - 1) / pl->TQ;
+  pl->n_split = attn_split_count(KV * B * pl->n_qtiles, max_ctx, n_sms);
   return 0;
+}
+
+// Varlen launch: sequences of one call have their own q_len and are packed row after row (sequence b owns rows
+// cu_q[b] .. cu_q[b+1]-1).  Each CTA tile is one entry of a tile table; a tile never crosses a sequence boundary.
+struct alignas(16) AttnTile {
+  int seq;   // sequence
+  int row0;  // first packed query row
+  int j0;    // index of that query inside its sequence (a multiple of TQ)
+  int tq;    // query rows of the tile
+};
+struct AttnVarlen {
+  const AttnTile* tiles;  // [n_tiles]
+  const int32_t* cu_q;    // [B + 1] prefix sums of q_len
+};
+// TQ and MT come from the longest q_len, n_split from KV * n_tiles CTAs; n_qtiles is the longest sequence's tile count,
+// so equal q_lens give exactly attn_make_plan's plan.  *n_tiles = sum_b ceil(q_len_b / TQ).
+inline int attn_make_plan_varlen(int H, int KV, int B, const int32_t* q_lens, int max_ctx, int n_sms, AttnPlan* pl,
+                                 int* n_tiles) {
+  int qmax = 0;
+  for (int b = 0; b < B; ++b) qmax = q_lens[b] > qmax ? q_lens[b] : qmax;
+  if (B < 1 || qmax < 1) return 3;
+  const int rc = attn_tile_shape(H, KV, qmax, pl);
+  if (rc != 0) return rc;
+  pl->n_qtiles = (qmax + pl->TQ - 1) / pl->TQ;
+  int nt = 0;
+  for (int b = 0; b < B; ++b) nt += (q_lens[b] + pl->TQ - 1) / pl->TQ;
+  *n_tiles = nt;
+  pl->n_split = attn_split_count(KV * nt, max_ctx, n_sms);
+  return 0;
+}
+// The tile table (in sequence order) and the prefix sums of a varlen plan; returns the number of tiles.
+inline int attn_varlen_tiles(int B, const int32_t* q_lens, int TQ, AttnTile* tiles, int32_t* cu_q) {
+  int nt = 0, row = 0;
+  for (int b = 0; b < B; ++b) {
+    cu_q[b] = row;
+    for (int j0 = 0; j0 < q_lens[b]; j0 += TQ) {
+      tiles[nt].seq = b;
+      tiles[nt].row0 = row + j0;
+      tiles[nt].j0 = j0;
+      tiles[nt].tq = q_lens[b] - j0 < TQ ? q_lens[b] - j0 : TQ;
+      ++nt;
+    }
+    row += q_lens[b];
+  }
+  cu_q[B] = row;
+  return nt;
 }
 // AttnParams::g_shift
 inline int attn_g_shift(int H, int KV) {
@@ -116,8 +170,10 @@ SSDK_DEVINL uint32_t pack_bf16x2(float lo, float hi) {
   return *reinterpret_cast<uint32_t*>(&v);
 }
 
-template <int HD, int MT>
-__global__ void __launch_bounds__(attn_warps(MT) * 32) paged_attn_kernel(AttnParams p) {
+// One CTA: kv head blockIdx.x, split blockIdx.y, query tile blockIdx.z (of a uniform launch, or an entry of the varlen
+// tile table).
+template <int HD, int MT, bool VARLEN>
+SSDK_DEVINL void paged_attn_cta(const AttnParams& p, const AttnVarlen& v) {
   constexpr int NW = attn_warps(MT);
   constexpr int kAttThreads = NW * 32;
   constexpr int LDS = HD + 8;               // padded smem row (bf16 elements)
@@ -137,12 +193,15 @@ __global__ void __launch_bounds__(attn_warps(MT) * 32) paged_attn_kernel(AttnPar
   if (threadIdx.x == 0) trace_mark(TR_ATTN);
 
   const int kvh = blockIdx.x, split = blockIdx.y;
-  const int b = blockIdx.z / p.n_qtiles, qt = blockIdx.z % p.n_qtiles;
+  // varlen: tile = table entry; qt * TQ is the tile's first query index j0 inside its sequence, q_len and the first
+  // packed row of the sequence come from the prefix sums
+  const int b = VARLEN ? v.tiles[blockIdx.z].seq : blockIdx.z / p.n_qtiles;
+  const int qt = VARLEN ? v.tiles[blockIdx.z].j0 / p.TQ : blockIdx.z % p.n_qtiles;
   const int G = p.H / p.KV;
-  const int tq = min(p.TQ, p.Q - qt * p.TQ);
+  const int tq = VARLEN ? v.tiles[blockIdx.z].tq : min(p.TQ, p.Q - qt * p.TQ);
   const int R = G * tq;
   const int ctx = p.context_lens[b];
-  const int ctx0 = ctx - p.Q;                         // tokens before this forward
+  const int ctx0 = ctx - (VARLEN ? v.cu_q[b + 1] - v.cu_q[b] : p.Q);  // tokens before this forward
   const int kv_max = ctx0 + qt * p.TQ + tq;           // exclusive upper bound of visible kv for this q-tile
   const int nch_total = (kv_max + kAttChunk - 1) / kAttChunk;
   const int cps = (nch_total + p.n_split - 1) / p.n_split;
@@ -162,8 +221,8 @@ __global__ void __launch_bounds__(attn_warps(MT) * 32) paged_attn_kernel(AttnPar
     const int r0 = mtile * 16 + g, r1 = r0 + 8;
     const __nv_bfloat16* q0 = nullptr;
     const __nv_bfloat16* q1 = nullptr;
-    if (r0 < R) q0 = p.q + ((size_t)(b * p.Q + qt * p.TQ + r0 / G) * p.H + kvh * G + r0 % G) * HD;
-    if (r1 < R) q1 = p.q + ((size_t)(b * p.Q + qt * p.TQ + r1 / G) * p.H + kvh * G + r1 % G) * HD;
+    if (r0 < R) q0 = p.q + ((size_t)((VARLEN ? v.cu_q[b] : b * p.Q) + qt * p.TQ + r0 / G) * p.H + kvh * G + r0 % G) * HD;
+    if (r1 < R) q1 = p.q + ((size_t)((VARLEN ? v.cu_q[b] : b * p.Q) + qt * p.TQ + r1 / G) * p.H + kvh * G + r1 % G) * HD;
 #pragma unroll
     for (int kk = 0; kk < KS; ++kk) {
       const int c = kk * 16 + 2 * t;
@@ -368,7 +427,7 @@ __global__ void __launch_bounds__(attn_warps(MT) * 32) paged_attn_kernel(AttnPar
       }
     }
     const int rt = (p.g_shift >= 0) ? (r >> p.g_shift) : r / G;  // token inside the tile; r - rt * G = head of the group
-    const int row_q = b * p.Q + qt * p.TQ + rt;
+    const int row_q = (VARLEN ? v.cu_q[b] : b * p.Q) + qt * p.TQ + rt;
     const int head = kvh * G + (r - rt * G);
     const float inv = (l > 0.f) ? 1.f / l : 0.f;
     acc.x *= inv; acc.y *= inv; acc.z *= inv; acc.w *= inv;
@@ -385,21 +444,45 @@ __global__ void __launch_bounds__(attn_warps(MT) * 32) paged_attn_kernel(AttnPar
   if (threadIdx.x == 0) trace_fine(TRF_ATTN + 3);  // partials / output stored
 }
 
+template <int HD, int MT>
+__global__ void __launch_bounds__(attn_warps(MT) * 32) paged_attn_kernel(AttnParams p) {
+  paged_attn_cta<HD, MT, false>(p, AttnVarlen{});
+}
+// p.B sequences packed by v.cu_q, grid.z = the tile table's length; p.Q and p.n_qtiles are unused
+template <int HD, int MT>
+__global__ void __launch_bounds__(attn_warps(MT) * 32) paged_attn_varlen_kernel(AttnParams p, AttnVarlen v) {
+  paged_attn_cta<HD, MT, true>(p, v);
+}
+
+// Sequence of packed row `tok` of a varlen launch: the b with cu_q[b] <= tok < cu_q[b + 1].
+SSDK_DEVINL int attn_varlen_seq(const int32_t* cu_q, int B, int tok) {
+  int lo = 0, hi = B - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (cu_q[mid] <= tok) lo = mid; else hi = mid - 1;
+  }
+  return lo;
+}
+
 // merge split-KV partials: out = sum_s 2^(lse_s - max) o_s / sum_s 2^(lse_s - max).
 // One CTA per (token, head) row, HD/4 threads, each owning one float4 of the output.  Only the splits that had
 // chunks (n_active, recomputed from context_lens with the attention kernel's formula) are read, and every thread
 // issues all of its loads before using them, so the merge costs ~2 L2 round trips whatever n_split is.
-__global__ void attn_combine_kernel(AttnParams p, int hd) {
+// VARLEN (p.B sequences packed by vl.cu_q, p.Q unused): the row's sequence comes from the prefix sums and its tile
+// starts at j rounded down to TQ, as attn_varlen_tiles lays the tiles out.  The uniform launch passes an empty vl.
+template <bool VARLEN>
+__global__ void attn_combine_kernel(AttnParams p, int hd, AttnVarlen vl) {
   SSDK_STATIC_SMEM(float, sw, 32);
   pdl_launch_dependents();
   pdl_wait();
   if (threadIdx.x == 0) trace_mark(TR_ATTN);
   const size_t row = blockIdx.x;  // (token, head)
   const int tok = (int)(row / p.H);
-  const int b = tok / p.Q, j = tok - b * p.Q;
+  const int b = VARLEN ? attn_varlen_seq(vl.cu_q, p.B, tok) : tok / p.Q, j = tok - (VARLEN ? vl.cu_q[b] : b * p.Q);
+  const int Q = VARLEN ? vl.cu_q[b + 1] - vl.cu_q[b] : p.Q;
   const int qt = j / p.TQ;
-  const int tq = min(p.TQ, p.Q - qt * p.TQ);
-  const int kv_max = p.context_lens[b] - p.Q + qt * p.TQ + tq;
+  const int tq = min(p.TQ, Q - qt * p.TQ);
+  const int kv_max = p.context_lens[b] - Q + qt * p.TQ + tq;
   const int nch_total = (kv_max + kAttChunk - 1) / kAttChunk;
   const int cps = (nch_total + p.n_split - 1) / p.n_split;
   const int n_active = (cps > 0) ? min(p.n_split, (nch_total + cps - 1) / cps) : 0;
@@ -441,5 +524,10 @@ __global__ void attn_combine_kernel(AttnParams p, int hd) {
   *reinterpret_cast<__nv_bfloat162*>(dst + 2) = __floats2bfloat162_rn(acc.z, acc.w);
   if (threadIdx.x == 0) trace_fine(TRF_COMB + 1);
 }
+
+#ifdef SSDK_HOST_EMU
+// host-thread drivers launch the uniform merge by its two arguments
+inline void attn_combine_kernel(const AttnParams& p, int hd) { attn_combine_kernel<false>(p, hd, AttnVarlen{}); }
+#endif
 
 }  // namespace ssdk

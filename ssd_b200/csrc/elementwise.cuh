@@ -125,6 +125,28 @@ __global__ void prep_kernel(const int32_t* __restrict__ ctx0, const int32_t* __r
   if (fwd_seq && i == 0) *fwd_seq += 1u;  // epoch base of this forward's one-shot all-reduces (tensor parallel target)
 }
 
+// prep_kernel for a varlen forward: sequence b owns packed rows cu_q[b] .. cu_q[b+1]-1, appended at ctx0[b].
+// One CTA of kMaxTokens threads, one per row.
+__global__ void prep_varlen_kernel(const int32_t* __restrict__ ctx0, const int32_t* __restrict__ cu_q,
+                                   const int32_t* __restrict__ block_tables, int max_blocks, int block_size, int batch,
+                                   int64_t* __restrict__ positions, int32_t* __restrict__ slot_mapping,
+                                   int32_t* __restrict__ context_lens, unsigned* __restrict__ fwd_seq) {
+  pdl_launch_dependents();
+  pdl_wait();
+  if (threadIdx.x == 0) trace_mark(TR_PREP);
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < cu_q[batch]) {
+    int b = 0;
+    while (cu_q[b + 1] <= i) ++b;
+    const int pos = ctx0[b] + i - cu_q[b];
+    positions[i] = pos;
+    const int blk = block_tables[(size_t)b * max_blocks + pos / block_size];
+    slot_mapping[i] = (blk < 0) ? -1 : blk * block_size + pos % block_size;
+  }
+  if (i < batch) context_lens[i] = ctx0[i] + cu_q[i + 1] - cu_q[i];
+  if (fwd_seq && i == 0) *fwd_seq += 1u;
+}
+
 // ----------------------------------------------------------------------------------
 // (embedding gather |) (split-K reduce |) residual add + RMSNorm.   grid = M rows.
 //   x row      = embed[ids[m*ids_stride] - vocab_start]  (ids != nullptr; rows outside the
@@ -531,6 +553,18 @@ __global__ void gather_last_rows_kernel(const __nv_bfloat16* __restrict__ x, __n
   if (threadIdx.x == 0) trace_mark(TR_MISC);
   const int b = blockIdx.x;
   const uint4* src = reinterpret_cast<const uint4*>(x + ((size_t)b * q_len + q_len - 1) * d);
+  uint4* dst = reinterpret_cast<uint4*>(out + (size_t)b * d);
+  for (int i = threadIdx.x; i < d / 8; i += blockDim.x) dst[i] = src[i];
+}
+
+// varlen forward: the last row of sequence b is packed row cu_q[b+1] - 1
+__global__ void gather_last_rows_varlen_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__ out,
+                                               const int32_t* __restrict__ cu_q, int d) {
+  pdl_launch_dependents();
+  pdl_wait();
+  if (threadIdx.x == 0) trace_mark(TR_MISC);
+  const int b = blockIdx.x;
+  const uint4* src = reinterpret_cast<const uint4*>(x + (size_t)(cu_q[b + 1] - 1) * d);
   uint4* dst = reinterpret_cast<uint4*>(out + (size_t)b * d);
   for (int i = threadIdx.x; i < d / 8; i += blockDim.x) dst[i] = src[i];
 }

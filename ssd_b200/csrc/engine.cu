@@ -261,7 +261,9 @@ struct Workspace {
   // step state
   uint8_t* out_dev;     // [tok_buf | n_accept | recovery] — one D2H per step
   int64_t* tok_buf;     // [max_batch, K+1]
-  int64_t* ids_in;      // [kMaxTokens]  (forward_tokens input)
+  int64_t* ids_in;      // [kMaxTokens]  (forward_tokens input), followed by the varlen inputs (kFwIn*)
+  int32_t* var_cu_q;    // [kMaxTokens + 1]  (forward_varlen prefix sums of q_len)
+  AttnTile* var_tiles;  // [kMaxTokens]      (forward_varlen attention tile table)
   int64_t* out_tok;     // [max_batch]   (forward_tokens sampled output)
   bf16 *logits_q, *logits_p, *logits_last;
   bf16 *logits_shard, *logits_gather;  // tensor-parallel lm_head: local [rows, V/tp] and all-gathered [tp, rows, V/tp]
@@ -286,6 +288,10 @@ struct Workspace {
 };
 
 constexpr int kSampleChunks = 64;
+// forward inputs, staged through one pinned ring slot and copied in one H2D: ids | cu_q | varlen tile table
+constexpr size_t kFwInCuOff = (size_t)kMaxTokens * 8;
+constexpr size_t kFwInTileOff = kFwInCuOff + ((size_t)(kMaxTokens + 1) * 4 + 15) / 16 * 16;
+constexpr size_t kFwInBytes = kFwInTileOff + (size_t)kMaxTokens * sizeof(AttnTile);
 constexpr int kLogCap = 16384;
 constexpr int kVerifyCtas = 128;
 
@@ -399,7 +405,9 @@ static int64_t carve(ssdk_engine* e, uint8_t* base) {
   w.recovery = (int64_t*)(w.out_dev ? w.out_dev + e->off_out_rec : nullptr);
   w.log_tokens = (int64_t*)take((size_t)MB * kLogCap * 8);
   w.log_len = (int32_t*)take((size_t)MB * 4);
-  w.ids_in = (int64_t*)take(kMaxTokens * 8);
+  w.ids_in = (int64_t*)take(kFwInBytes);
+  w.var_cu_q = (int32_t*)(w.ids_in ? (uint8_t*)w.ids_in + kFwInCuOff : nullptr);
+  w.var_tiles = (AttnTile*)(w.ids_in ? (uint8_t*)w.ids_in + kFwInTileOff : nullptr);
   w.out_tok = (int64_t*)take(kMaxTokens * 8);
   w.logits_q = (bf16*)take((size_t)MB * std::max(K, 1) * vmax * 2);
   w.logits_p = (bf16*)take((size_t)MB * (K + 1) * vmax * 2);
@@ -421,6 +429,13 @@ static int64_t carve(ssdk_engine* e, uint8_t* base) {
 // ------------------------------------------------------------------------------------------
 // one forward pass (enqueue only)
 // ------------------------------------------------------------------------------------------
+// a varlen forward (ssdk_forward_varlen): prefix sums and attention tiles on the device, the plan made on the host
+struct VarlenFwd {
+  AttnVarlen attn;
+  AttnPlan plan;
+  int n_tiles;
+  int M;
+};
 struct Fwd {
   int which;
   int B, Q;
@@ -432,6 +447,7 @@ struct Fwd {
   int logits_mode;  // 0 none, 1 all rows, 2 last row per sequence
   bf16* logits_out;
   int64_t logits_ld;
+  const VarlenFwd* var = nullptr;  // set: B sequences of their own q_len packed into M rows (Q unused)
 };
 
 static int attn_plan_raw(int H, int KV, int B, int Q, int max_ctx, int* TQ, int* MT, int* nqt, int* nsplit) {
@@ -450,22 +466,24 @@ static int attn_plan(const Model& m, int B, int Q, int* TQ, int* MT, int* nqt, i
 }
 
 template <int HD, int MT>
-static int launch_attn_inst(Launcher& L, const AttnParams& p, dim3 grid) {
+static int launch_attn_inst(Launcher& L, const AttnParams& p, const AttnVarlen* var, dim3 grid) {
   const size_t smem = (size_t)2 * 2 * kAttChunk * (HD + 8) * 2;
   static bool attr_set = false;
   if (!attr_set) {
     CK(cudaFuncSetAttribute(paged_attn_kernel<HD, MT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CK(cudaFuncSetAttribute(paged_attn_varlen_kernel<HD, MT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr_set = true;
   }
+  if (var) return L.go(paged_attn_varlen_kernel<HD, MT>, grid, dim3(attn_warps(MT) * 32), smem, p, *var);
   return L.go(paged_attn_kernel<HD, MT>, grid, dim3(attn_warps(MT) * 32), smem, p);
 }
-static int launch_attn(Launcher& L, const AttnParams& p, int hd, int MT, dim3 grid) {
-  if (hd == 128 && MT == 1) return launch_attn_inst<128, 1>(L, p, grid);
-  if (hd == 128 && MT == 2) return launch_attn_inst<128, 2>(L, p, grid);
-  if (hd == 128 && MT == 4) return launch_attn_inst<128, 4>(L, p, grid);
-  if (hd == 64 && MT == 1) return launch_attn_inst<64, 1>(L, p, grid);
-  if (hd == 64 && MT == 2) return launch_attn_inst<64, 2>(L, p, grid);
-  if (hd == 64 && MT == 4) return launch_attn_inst<64, 4>(L, p, grid);
+static int launch_attn(Launcher& L, const AttnParams& p, const AttnVarlen* var, int hd, int MT, dim3 grid) {
+  if (hd == 128 && MT == 1) return launch_attn_inst<128, 1>(L, p, var, grid);
+  if (hd == 128 && MT == 2) return launch_attn_inst<128, 2>(L, p, var, grid);
+  if (hd == 128 && MT == 4) return launch_attn_inst<128, 4>(L, p, var, grid);
+  if (hd == 64 && MT == 1) return launch_attn_inst<64, 1>(L, p, var, grid);
+  if (hd == 64 && MT == 2) return launch_attn_inst<64, 2>(L, p, var, grid);
+  if (hd == 64 && MT == 4) return launch_attn_inst<64, 4>(L, p, var, grid);
   return fail("unsupported head_dim %d (64 and 128 are built)", hd);
 }
 
@@ -473,7 +491,7 @@ static int enqueue_attention(Launcher& L, const bf16* q, const bf16* kc, const b
                              const int32_t* ctx_lens, bf16* out, float* part_o, float* part_lse, unsigned* counters,
                              int B, int Q, int H,
                              int KV, int hd, int block_size, int max_blocks, float scale, int TQ, int MT, int nqt,
-                             int nsplit) {
+                             int nsplit, const VarlenFwd* var = nullptr) {
   AttnParams a;
   a.q = q; a.k_cache = kc; a.v_cache = vc; a.block_tables = bt; a.context_lens = ctx_lens; a.out = out;
   a.part_o = part_o; a.part_lse = part_lse;
@@ -482,8 +500,13 @@ static int enqueue_attention(Launcher& L, const bf16* q, const bf16* kc, const b
   a.n_split = nsplit; a.TQ = TQ; a.n_qtiles = nqt;
   a.g_shift = attn_g_shift(H, KV);
   a.scale_log2 = scale * 1.4426950408889634f;
-  CKI(launch_attn(L, a, hd, MT, dim3(KV, nsplit, B * nqt)));
-  if (nsplit > 1) CKI(L.go(attn_combine_kernel, dim3(B * Q * H), dim3(32), 0, a, hd));
+  if (var) {
+    CKI(launch_attn(L, a, &var->attn, hd, MT, dim3(KV, nsplit, var->n_tiles)));
+    if (nsplit > 1) CKI(L.go(attn_combine_kernel<true>, dim3(var->M * H), dim3(32), 0, a, hd, var->attn));
+    return 0;
+  }
+  CKI(launch_attn(L, a, nullptr, hd, MT, dim3(KV, nsplit, B * nqt)));
+  if (nsplit > 1) CKI(L.go(attn_combine_kernel<false>, dim3(B * Q * H), dim3(32), 0, a, hd, AttnVarlen{}));
   return 0;
 }
 
@@ -621,19 +644,24 @@ __global__ void unshard_logits_kernel(const bf16* __restrict__ gathered, bf16* _
 static int enqueue_forward(ssdk_engine* e, Launcher& L, const Fwd& f) {
   Model& m = e->model[f.which];
   Workspace& w = e->ws;
-  const int M = f.B * f.Q;
+  const int M = f.var ? f.var->M : f.B * f.Q;
   if (M < 1 || M > kMaxTokens) return fail("forward: %d tokens (max %d)", M, kMaxTokens);
   const int tp = m.cfg.tp_size;
   if (tp > 1 && !e->comm) return fail("tensor parallel forward without a NCCL communicator");
   const int bs = e->rt.block_size, mb = e->rt.max_blocks_per_seq;
   const int64_t cache_layer_stride = m.num_blocks * bs * m.KV * m.hd;
 
-  CKI(L.go(prep_kernel, dim3(1), dim3(kMaxTokens), 0, f.ctx0, f.block_tables, mb, bs, f.B, f.Q, f.pos_offset,
-           w.positions, w.slot_mapping, w.context_lens,
-           (f.which == SSDK_TARGET && tp > 1 && e->symm_n == tp) ? w.ar_state : (unsigned*)nullptr));
-
+  unsigned* fwd_seq = (f.which == SSDK_TARGET && tp > 1 && e->symm_n == tp) ? w.ar_state : (unsigned*)nullptr;
   int TQ = 1, MT = 1, nqt = 1, nsplit = 1;
-  CKI(attn_plan(m, f.B, f.Q, &TQ, &MT, &nqt, &nsplit, e->max_ctx_hint));
+  if (f.var) {
+    CKI(L.go(prep_varlen_kernel, dim3(1), dim3(kMaxTokens), 0, f.ctx0, f.var->attn.cu_q, f.block_tables, mb, bs, f.B,
+             w.positions, w.slot_mapping, w.context_lens, fwd_seq));
+    TQ = f.var->plan.TQ; MT = f.var->plan.MT; nqt = f.var->plan.n_qtiles; nsplit = f.var->plan.n_split;
+  } else {
+    CKI(L.go(prep_kernel, dim3(1), dim3(kMaxTokens), 0, f.ctx0, f.block_tables, mb, bs, f.B, f.Q, f.pos_offset,
+             w.positions, w.slot_mapping, w.context_lens, fwd_seq));
+    CKI(attn_plan(m, f.B, f.Q, &TQ, &MT, &nqt, &nsplit, e->max_ctx_hint));
+  }
   const float scale = 1.0f / sqrtf((float)m.hd);
 
   const bool use_symm = tp > 1 && e->symm_n == tp;
@@ -693,7 +721,8 @@ static int enqueue_forward(ssdk_engine* e, Launcher& L, const Fwd& f) {
 
     // ---- attention over the paged cache ----
     CKI(enqueue_attention(L, w.q, rp.k_cache, rp.v_cache, f.block_tables, w.context_lens, w.attn_out, w.att_o,
-                          w.att_lse, w.att_counters, f.B, f.Q, m.H, m.KV, m.hd, bs, mb, scale, TQ, MT, nqt, nsplit));
+                          w.att_lse, w.att_counters, f.B, f.Q, m.H, m.KV, m.hd, bs, mb, scale, TQ, MT, nqt, nsplit,
+                          f.var));
 
     // ---- output projection (row-parallel) ----
     const bool fuse_pub = use_symm && fused_publish_enabled() && M <= 64;
@@ -760,7 +789,14 @@ static int enqueue_forward(ssdk_engine* e, Launcher& L, const Fwd& f) {
   if (f.logits_mode != 0) {
     const bf16* x = w.hidden;
     int rows = M;
-    if (f.logits_mode == 2 && f.Q > 1) {
+    if (f.logits_mode == 2 && f.var) {
+      if (M > f.B) {
+        CKI(L.go(gather_last_rows_varlen_kernel, dim3(f.B), dim3(256), 0, (const bf16*)w.hidden, w.last_hidden,
+                 f.var->attn.cu_q, m.d));
+        x = w.last_hidden;
+      }
+      rows = f.B;
+    } else if (f.logits_mode == 2 && f.Q > 1) {
       CKI(L.go(gather_last_rows_kernel, dim3(f.B), dim3(256), 0, (const bf16*)w.hidden, w.last_hidden, f.B, f.Q, m.d));
       x = w.last_hidden;
       rows = f.B;
@@ -1077,6 +1113,10 @@ static int init_kernel_attrs() {
   CK(cudaFuncSetAttribute(paged_attn_kernel<HD, MT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * 2 * kAttChunk * (HD + 8) * 2));
   SSDK_ATTR_A(128, 1) SSDK_ATTR_A(128, 2) SSDK_ATTR_A(128, 4) SSDK_ATTR_A(64, 1) SSDK_ATTR_A(64, 2) SSDK_ATTR_A(64, 4)
 #undef SSDK_ATTR_A
+#define SSDK_ATTR_AV(HD, MT) \
+  CK(cudaFuncSetAttribute(paged_attn_varlen_kernel<HD, MT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * 2 * kAttChunk * (HD + 8) * 2));
+  SSDK_ATTR_AV(128, 1) SSDK_ATTR_AV(128, 2) SSDK_ATTR_AV(128, 4) SSDK_ATTR_AV(64, 1) SSDK_ATTR_AV(64, 2) SSDK_ATTR_AV(64, 4)
+#undef SSDK_ATTR_AV
   CK(cudaFuncSetAttribute(add_rmsnorm_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
   return 0;
 }
@@ -1144,7 +1184,7 @@ int ssdk_create(const ssdk_model_cfg* target, const ssdk_model_cfg* draft, const
     return fail("pinned staging allocation failed");
   }
   memset(e->pin_in, 0, e->step_bytes);
-  e->fw_slot_bytes = align_up(e->step_bytes, 64) + (size_t)kMaxTokens * 8;
+  e->fw_slot_bytes = align_up(e->step_bytes, 64) + kFwInBytes;
   if (cudaHostAlloc((void**)&e->pin_fw, e->fw_slot_bytes * ssdk_engine::kFwSlots, cudaHostAllocDefault) != cudaSuccess) {
     cudaFreeHost(e->pin_in);
     cudaFreeHost(e->pin_out);
@@ -1411,16 +1451,29 @@ int ssdk_spec_step_log(ssdk_handle h, int seq, int64_t* out_tokens, int cap, voi
   return n;
 }
 
-int ssdk_forward_tokens(ssdk_handle h, int which, int batch, int q_len, const int64_t* ids, const int32_t* ctx_len,
-                        const int32_t* block_tables, int want_sample, const float* temps, uint64_t seed,
-                        uint64_t step_id, int64_t* out_tokens, void* stream) {
-  if (!h || !h->finalized) return fail("forward_tokens: engine not finalized");
-  if (which < 0 || which > 1 || !h->model[which].present) return fail("forward_tokens: model %d absent", which);
-  if (batch < 1 || batch > h->rt.max_batch || q_len < 1 || batch * q_len > kMaxTokens)
-    return fail("forward_tokens: batch=%d q_len=%d out of range", batch, q_len);
+// ssdk_forward_tokens (q_lens == nullptr: q_len tokens per sequence) and ssdk_forward_varlen (q_lens[b] tokens of
+// sequence b, packed).  Arguments are checked by the callers.
+static int forward_call(ssdk_handle h, int which, int batch, int q_len, const int32_t* q_lens, const int64_t* ids,
+                        const int32_t* ctx_len, const int32_t* block_tables, int want_sample, const float* temps,
+                        uint64_t seed, uint64_t step_id, int64_t* out_tokens, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   Workspace& w = h->ws;
+  Model& m = h->model[which];
   const int mbk = h->rt.max_blocks_per_seq;
+  VarlenFwd var;
+  int M = batch * q_len;
+  if (q_lens) {
+    int32_t n_tiles = 0;
+    const int rc = attn_make_plan_varlen(m.H, m.KV, batch, q_lens, h->max_ctx_hint, num_sms(), &var.plan, &n_tiles);
+    if (rc == 1) return fail("unsupported GQA ratio %d/%d", m.H, m.KV);
+    if (rc != 0) return fail("attention tile too large");
+    var.n_tiles = n_tiles;
+    M = 0;
+    for (int b = 0; b < batch; ++b) M += q_lens[b];
+    var.M = M;
+    var.attn.cu_q = w.var_cu_q;
+    var.attn.tiles = w.var_tiles;
+  }
   // stage inputs through one slot of the pinned ring (block tables go to the step-block field of `which`); wait for the
   // copies that last read this slot before overwriting it — a non-sampling call returns without synchronizing, and its
   // H2D copies are queued behind the previous chunk's kernels
@@ -1437,9 +1490,14 @@ int ssdk_forward_tokens(ssdk_handle h, int which, int batch, int q_len, const in
   memcpy(pin + h->off_seed, ss, 16);
   memcpy(pin + (which == SSDK_TARGET ? h->off_btt : h->off_btd), block_tables, (size_t)batch * mbk * 4);
   CK(cudaMemcpyAsync(w.step_dev, pin, h->step_bytes, cudaMemcpyHostToDevice, st));
-  int64_t* pin_ids_in = (int64_t*)(pin + align_up(h->step_bytes, 64));
-  memcpy(pin_ids_in, ids, (size_t)batch * q_len * 8);
-  CK(cudaMemcpyAsync(w.ids_in, pin_ids_in, (size_t)batch * q_len * 8, cudaMemcpyHostToDevice, st));
+  uint8_t* pin_in = pin + align_up(h->step_bytes, 64);  // ids | cu_q | tile table, as w.ids_in
+  memcpy(pin_in, ids, (size_t)M * 8);
+  size_t in_bytes = (size_t)M * 8;
+  if (q_lens) {
+    attn_varlen_tiles(batch, q_lens, var.plan.TQ, (AttnTile*)(pin_in + kFwInTileOff), (int32_t*)(pin_in + kFwInCuOff));
+    in_bytes = kFwInTileOff + (size_t)var.n_tiles * sizeof(AttnTile);
+  }
+  CK(cudaMemcpyAsync(w.ids_in, pin_in, in_bytes, cudaMemcpyHostToDevice, st));
   CK(cudaEventRecord(h->fw_ev[slot], st));
   h->fw_ev_pending[slot] = true;
   // sampled tokens come back through the tail of the result staging buffer (read after the synchronize below)
@@ -1448,7 +1506,6 @@ int ssdk_forward_tokens(ssdk_handle h, int which, int batch, int q_len, const in
   Launcher L;
   L.st = st;
   L.pdl = h->rt.use_pdl != 0;
-  Model& m = h->model[which];
   Fwd f;
   f.which = which; f.B = batch; f.Q = q_len; f.ids = w.ids_in; f.ids_stride = 1;
   f.ctx0 = (const int32_t*)(w.step_dev + h->off_ctx);
@@ -1457,6 +1514,7 @@ int ssdk_forward_tokens(ssdk_handle h, int which, int batch, int q_len, const in
   f.logits_mode = want_sample ? 2 : 0;
   f.logits_out = w.logits_last;
   f.logits_ld = m.cfg.vocab;
+  f.var = q_lens ? &var : nullptr;
   CKI(enqueue_forward(h, L, f));
   const bool do_sample = want_sample && m.cfg.tp_rank == 0;
   if (do_sample) {
@@ -1474,6 +1532,35 @@ int ssdk_forward_tokens(ssdk_handle h, int which, int batch, int q_len, const in
   }
   h->launches += L.count;
   return 0;
+}
+
+int ssdk_forward_tokens(ssdk_handle h, int which, int batch, int q_len, const int64_t* ids, const int32_t* ctx_len,
+                        const int32_t* block_tables, int want_sample, const float* temps, uint64_t seed,
+                        uint64_t step_id, int64_t* out_tokens, void* stream) {
+  if (!h || !h->finalized) return fail("forward_tokens: engine not finalized");
+  if (which < 0 || which > 1 || !h->model[which].present) return fail("forward_tokens: model %d absent", which);
+  if (batch < 1 || batch > h->rt.max_batch || q_len < 1 || batch * q_len > kMaxTokens)
+    return fail("forward_tokens: batch=%d q_len=%d out of range", batch, q_len);
+  return forward_call(h, which, batch, q_len, nullptr, ids, ctx_len, block_tables, want_sample, temps, seed, step_id,
+                      out_tokens, stream);
+}
+
+int ssdk_forward_varlen(ssdk_handle h, int which, int n_seqs, const int32_t* q_lens, const int64_t* ids,
+                        const int32_t* ctx_len, const int32_t* block_tables, int want_sample, const float* temps,
+                        uint64_t seed, uint64_t step_id, int64_t* out_tokens, void* stream) {
+  if (!h || !h->finalized) return fail("forward_varlen: engine not finalized");
+  if (which < 0 || which > 1 || !h->model[which].present) return fail("forward_varlen: model %d absent", which);
+  if (n_seqs < 1 || n_seqs > h->rt.max_batch)
+    return fail("forward_varlen: n_seqs=%d out of range [1, %d]", n_seqs, h->rt.max_batch);
+  if (!q_lens || !ids || !ctx_len || !block_tables) return fail("forward_varlen: null argument");
+  int total = 0;
+  for (int b = 0; b < n_seqs; ++b) {
+    if (q_lens[b] < 1) return fail("forward_varlen: q_lens[%d]=%d < 1", b, q_lens[b]);
+    total += q_lens[b];
+    if (total > kMaxTokens) return fail("forward_varlen: more than %d tokens in one call", kMaxTokens);
+  }
+  return forward_call(h, which, n_seqs, 0, q_lens, ids, ctx_len, block_tables, want_sample, temps, seed, step_id,
+                      out_tokens, stream);
 }
 
 // debug: route the kernels' timeline marks into `dev_buf` (uint64 [cap][2]); dev_buf = NULL disables tracing
@@ -1602,6 +1689,51 @@ int ssdk_paged_attn(const void* q, const void* k_cache, const void* v_cache, con
   return enqueue_attention(L, (const bf16*)q, (const bf16*)k_cache, (const bf16*)v_cache, block_tables, context_lens,
                            (bf16*)out, part_o, part_lse, (unsigned*)scratch, batch, q_len, heads, kv_heads, head_dim, block_size,
                            max_blocks_per_seq, scale, TQ, MT, nqt, nsplit);
+}
+
+int ssdk_paged_attn_varlen_plan(int heads, int kv_heads, int batch, const int32_t* q_lens, int max_ctx, int* out5) {
+  if (batch < 1 || batch > kMaxTokens || !q_lens || kv_heads < 1 || out5 == nullptr)
+    return fail("paged_attn_varlen_plan: bad arguments");
+  int total = 0;
+  for (int b = 0; b < batch; ++b) {
+    if (q_lens[b] < 1) return fail("paged_attn_varlen_plan: q_lens[%d]=%d < 1", b, q_lens[b]);
+    total += q_lens[b];
+  }
+  if (total > kMaxTokens) return fail("paged_attn_varlen_plan: %d query tokens (max %d)", total, kMaxTokens);
+  AttnPlan pl;
+  const int rc = attn_make_plan_varlen(heads, kv_heads, batch, q_lens, max_ctx, num_sms(), &pl, &out5[4]);
+  if (rc == 1) return fail("unsupported GQA ratio %d/%d", heads, kv_heads);
+  if (rc != 0) return fail("attention tile too large");
+  out5[0] = pl.TQ; out5[1] = pl.MT; out5[2] = pl.n_qtiles; out5[3] = pl.n_split;
+  return 0;
+}
+
+int ssdk_paged_attn_varlen(const void* q, const void* k_cache, const void* v_cache, const int32_t* block_tables,
+                           const int32_t* context_lens, const int32_t* q_lens, void* out, void* scratch, int batch,
+                           int heads, int kv_heads, int head_dim, int block_size, int max_blocks_per_seq, float scale,
+                           void* stream) {
+  int plan[5];
+  CKI(ssdk_paged_attn_varlen_plan(heads, kv_heads, batch, q_lens, block_size * max_blocks_per_seq, plan));
+  Launcher L;
+  L.st = (cudaStream_t)stream;
+  CKI(init_kernel_attrs());
+  // the first 16 KB of the scratch hold the prefix sums (at 0) and the tile table (at 8 KB)
+  int32_t cu_q[kMaxTokens + 1];
+  AttnTile tiles[kMaxTokens];
+  VarlenFwd var;
+  var.plan.TQ = plan[0]; var.plan.MT = plan[1]; var.plan.n_qtiles = plan[2]; var.plan.n_split = plan[3];
+  var.n_tiles = attn_varlen_tiles(batch, q_lens, plan[0], tiles, cu_q);
+  var.M = cu_q[batch];
+  var.attn.cu_q = (const int32_t*)scratch;
+  var.attn.tiles = (const AttnTile*)((uint8_t*)scratch + 8192);
+  CK(cudaMemcpyAsync(scratch, cu_q, (size_t)(batch + 1) * 4, cudaMemcpyHostToDevice, L.st));
+  CK(cudaMemcpyAsync((uint8_t*)scratch + 8192, tiles, (size_t)var.n_tiles * sizeof(AttnTile), cudaMemcpyHostToDevice, L.st));
+  L.barrier_op();
+  float* part_o = (float*)((uint8_t*)scratch + 16384);
+  float* part_lse = part_o + (size_t)var.M * heads * kAttnMaxSplit * head_dim;
+  return enqueue_attention(L, (const bf16*)q, (const bf16*)k_cache, (const bf16*)v_cache, block_tables, context_lens,
+                           (bf16*)out, part_o, part_lse, nullptr, batch, 0, heads, kv_heads, head_dim, block_size,
+                           max_blocks_per_seq, scale, var.plan.TQ, var.plan.MT, var.plan.n_qtiles, var.plan.n_split, &var);
 }
 
 int ssdk_sample(const void* logits, int64_t ld, const float* temps, int B, int V, uint64_t seed, uint64_t step_id,

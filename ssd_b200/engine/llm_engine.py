@@ -86,8 +86,10 @@ class LLMEngine:
 
     def create_inference_step(self, config: Config) -> InferenceStep:
         if config.speculate:
-            return SpecDecodeStep(self.scheduler, self.runner, config.speculate_k, METRICS, self.tokenizer, config.seed)
-        return AutoRegressiveStep(self.scheduler, self.runner, self.tokenizer, config.seed)
+            return SpecDecodeStep(self.scheduler, self.runner, config.speculate_k, METRICS, self.tokenizer, config.seed,
+                                  varlen_prefill=config.varlen_prefill)
+        return AutoRegressiveStep(self.scheduler, self.runner, self.tokenizer, config.seed,
+                                  varlen_prefill=config.varlen_prefill)
 
     def step(self, step: InferenceStep):
         t = perf_counter()

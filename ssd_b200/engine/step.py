@@ -28,14 +28,15 @@ class InferenceStep(ABC):
 class AutoRegressiveStep(InferenceStep):
     """engine/step.py:29-53."""
 
-    def __init__(self, scheduler, runner, tokenizer=None, seed: int = 0):
+    def __init__(self, scheduler, runner, tokenizer=None, seed: int = 0, varlen_prefill: bool = False):
         super().__init__(scheduler)
         self.runner, self.tokenizer, self.seed = runner, tokenizer, seed
+        self.prefill_fn = runner.prefill_varlen if varlen_prefill else runner.prefill_many
 
     def prefill(self, seqs) -> int:
-        toks = self.runner.prefill_many(L.TARGET, [s.token_ids for s in seqs], [s.block_table for s in seqs],
-                                        [min(s.num_cached_tokens, len(s) - 1) for s in seqs],
-                                        [s.temperature for s in seqs], seed=self.seed)
+        toks = self.prefill_fn(L.TARGET, [s.token_ids for s in seqs], [s.block_table for s in seqs],
+                               [min(s.num_cached_tokens, len(s) - 1) for s in seqs],
+                               [s.temperature for s in seqs], seed=self.seed)
         self.scheduler.postprocess(seqs, toks, True)
         return sum(len(s) for s in seqs)
 
@@ -49,20 +50,22 @@ class AutoRegressiveStep(InferenceStep):
 class SpecDecodeStep(InferenceStep):
     """engine/step.py:56-163 for synchronous speculation."""
 
-    def __init__(self, scheduler, runner, lookahead: int, metrics: dict, tokenizer=None, seed: int = 0):
+    def __init__(self, scheduler, runner, lookahead: int, metrics: dict, tokenizer=None, seed: int = 0,
+                 varlen_prefill: bool = False):
         super().__init__(scheduler)
         self.runner, self.K, self.metrics, self.tokenizer, self.seed = runner, lookahead, metrics, tokenizer, seed
+        self.prefill_fn = runner.prefill_varlen if varlen_prefill else runner.prefill_many
 
     def prefill(self, seqs) -> int:
         """Target prefill samples the first recovery token (verifier.py:32-52), then the draft caches the prompt
         (speculator_sync.py:14-23).  Prefix-cache hits skip the cached blocks (scheduler.py:71-72)."""
         ids = [s.token_ids for s in seqs]
         # always run at least the last token to get logits
-        rec = self.runner.prefill_many(L.TARGET, ids, [s.block_table for s in seqs],
-                                       [min(s.num_cached_tokens, len(s) - 1) for s in seqs],
-                                       [s.temperature for s in seqs], seed=self.seed)
-        self.runner.prefill_many(L.DRAFT, ids, [s.draft_block_table for s in seqs],
-                                 [min(s.num_draft_cached_tokens, len(s) - 1) for s in seqs], want_sample=False)
+        rec = self.prefill_fn(L.TARGET, ids, [s.block_table for s in seqs],
+                              [min(s.num_cached_tokens, len(s) - 1) for s in seqs],
+                              [s.temperature for s in seqs], seed=self.seed)
+        self.prefill_fn(L.DRAFT, ids, [s.draft_block_table for s in seqs],
+                        [min(s.num_draft_cached_tokens, len(s) - 1) for s in seqs], want_sample=False)
         for seq, r in zip(seqs, rec):
             seq.recovery_token_id = r
             seq.num_cached_tokens = seq.num_prompt_tokens

@@ -65,6 +65,8 @@ SIGNATURES: dict[str, tuple] = {
     "ssdk_spec_step_log": (C.c_int, [VP, C.c_int, c_i64p, C.c_int, VP]),
     "ssdk_forward_tokens": (C.c_int, [VP, C.c_int, C.c_int, C.c_int, c_i64p, c_i32p, c_i32p, C.c_int, c_f32p,
                                       C.c_uint64, C.c_uint64, c_i64p, VP]),
+    "ssdk_forward_varlen": (C.c_int, [VP, C.c_int, C.c_int, c_i32p, c_i64p, c_i32p, c_i32p, C.c_int, c_f32p,
+                                      C.c_uint64, C.c_uint64, c_i64p, VP]),
     "ssdk_logits_p": (VP, [VP]),
     "ssdk_logits_q": (VP, [VP]),
     "ssdk_logits_last": (VP, [VP]),
@@ -80,6 +82,9 @@ SIGNATURES: dict[str, tuple] = {
     "ssdk_paged_attn": (C.c_int, [VP, VP, VP, VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                   C.c_int, C.c_float, VP]),
     "ssdk_paged_attn_plan": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, c_i32p]),
+    "ssdk_paged_attn_varlen": (C.c_int, [VP, VP, VP, VP, VP, c_i32p, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                         C.c_int, C.c_float, VP]),
+    "ssdk_paged_attn_varlen_plan": (C.c_int, [C.c_int, C.c_int, C.c_int, c_i32p, C.c_int, c_i32p]),
     "ssdk_sample": (C.c_int, [VP, C.c_int64, VP, C.c_int, C.c_int, C.c_uint64, C.c_uint64, VP, VP]),
     "ssdk_verify_scratch_bytes": (C.c_int64, [C.c_int, C.c_int]),
     "ssdk_verify": (C.c_int, [VP, VP, VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_uint64, C.c_uint64,

@@ -149,6 +149,43 @@ def paged_attention_plan(B: int, q_len: int, H: int, KV: int, max_ctx: int) -> d
     return {"TQ": out[0], "MT": out[1], "n_qtiles": out[2], "n_split": out[3]}
 
 
+def paged_attention_varlen(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, block_tables: torch.Tensor,
+                           context_lens: torch.Tensor, q_lens: list[int], scale: float) -> torch.Tensor:
+    """flash_attn_varlen_func over the paged cache (layers/attention.py:85-93): sequence b has q_lens[b] queries, packed
+    in sequence order, and context_lens[b] includes them.
+
+    q [sum(q_lens), H, hd]; caches [num_blocks, block_size, KV, hd]; returns [sum(q_lens), H*hd]."""
+    _req(q, torch.bfloat16, "q")
+    _req(k_cache, torch.bfloat16, "k_cache")
+    _req(v_cache, torch.bfloat16, "v_cache")
+    _req(block_tables, torch.int32, "block_tables")
+    _req(context_lens, torch.int32, "context_lens")
+    Mq, H, hd = q.shape
+    B = len(q_lens)
+    assert sum(q_lens) == Mq and context_lens.shape[0] == B and block_tables.shape[0] == B
+    _, block_size, KV, _ = k_cache.shape
+    max_blocks = block_tables.shape[1]
+    ql = (C.c_int32 * B)(*q_lens)
+    lib = _L.load()
+    nbytes = lib.ssdk_paged_attn_scratch_bytes(1, Mq, H, hd, max_blocks * block_size)
+    scratch = torch.empty(nbytes, dtype=torch.uint8, device=q.device)
+    out = torch.empty(Mq, H * hd, dtype=torch.bfloat16, device=q.device)
+    _L.check(lib.ssdk_paged_attn_varlen(_ptr(q), _ptr(k_cache), _ptr(v_cache), _ptr(block_tables), _ptr(context_lens), ql,
+                                        _ptr(out), _ptr(scratch), B, H, KV, hd, block_size, max_blocks, float(scale),
+                                        _stream()), "ssdk_paged_attn_varlen")
+    return out
+
+
+def paged_attention_varlen_plan(q_lens: list[int], H: int, KV: int, max_ctx: int) -> dict:
+    """The launch plan paged_attention_varlen takes: paged_attention_plan's fields (n_qtiles of the longest sequence)
+    plus the number of query tiles in the launch."""
+    out = (C.c_int32 * 5)()
+    ql = (C.c_int32 * len(q_lens))(*q_lens)
+    lib = _L.load()
+    _L.check(lib.ssdk_paged_attn_varlen_plan(H, KV, len(q_lens), ql, max_ctx, out), "ssdk_paged_attn_varlen_plan")
+    return {"TQ": out[0], "MT": out[1], "n_qtiles": out[2], "n_split": out[3], "n_tiles": out[4]}
+
+
 def sample(logits: torch.Tensor, temperatures: torch.Tensor, seed: int = 0, step_id: int = 0) -> torch.Tensor:
     """Sampler.forward (layers/sampler.py:14-36) — logits [B, V] bf16, temperatures [B] fp32 -> int64 [B]."""
     _req(logits, torch.bfloat16, "logits")

@@ -244,6 +244,91 @@ class PairRunner:
                                       want_sample=want_sample, chunk=chunk, seed=seed)
         return out if want_sample else None
 
+    def forward_varlen(self, which: int, ids: list[list[int]], ctx_len: list[int], block_tables, temps=None,
+                       want_sample: bool = True, seed: int = 0) -> list[int] | None:
+        """forward_tokens for sequences of different lengths in one call (ssdk_forward_varlen): ids[b] is appended at
+        ctx_len[b]; with want_sample, the last row of every sequence is sampled."""
+        if self.spec[which] is None:
+            return None
+        B = len(ids)
+        q_a = _i32([len(x) for x in ids])
+        ids_a = np.ascontiguousarray(np.fromiter((t for x in ids for t in x), dtype=np.int64, count=int(q_a.sum())))
+        ctx_a, bt_a = _i32(ctx_len), self._bt(block_tables)
+        temps_a = np.ascontiguousarray(temps if temps is not None else [0.0] * B, dtype=np.float32)
+        out = np.zeros(B, dtype=np.int64)
+        st = torch.cuda.current_stream().cuda_stream
+        L.check(self.lib.ssdk_forward_varlen(self.h, which, B, q_a.ctypes.data_as(L.c_i32p), ids_a.ctypes.data_as(L.c_i64p),
+                                             ctx_a.ctypes.data_as(L.c_i32p), bt_a.ctypes.data_as(L.c_i32p),
+                                             int(want_sample), temps_a.ctypes.data_as(L.c_f32p), seed, self.step_id,
+                                             out.ctypes.data_as(L.c_i64p), st), "ssdk_forward_varlen")
+        self.step_id += 1
+        return out.tolist() if want_sample else None
+
+    @staticmethod
+    def plan_varlen_calls(lens: list[int], starts: list[int], block_tables: list[list[int]], block_size: int,
+                          max_tokens: int = 256, max_batch: int = 32) -> list[list[tuple[int, int, int]]]:
+        """The varlen prefill calls of one batch: each call is a list of (sequence, first position, tokens), in sequence
+        order.  Calls are filled in sequence order up to max_tokens tokens and max_batch sequences; a prompt longer than
+        what is left of a call continues in the next one.
+
+        Prefix-cache hits (start > 0) read the K/V of pages that another sequence of the batch may still be writing
+        (block_manager hashes a block when it is allocated).  A hit i may have tokens in a call only if every other
+        sequence j holding one of i's first ceil(start_i / block_size) pages has computed min(start_i, len_j) tokens by the
+        end of that call.  Tokens of j in the SAME call count: inside a forward, each layer stores the K/V of all rows of
+        the call before that layer's attention runs, so i's attention already sees what j writes in this call.
+        Two hits never wait on each other: the one with the larger start has already computed what the other needs, so
+        some sequence can always run and the loop ends."""
+        n = len(lens)
+        done = [min(s, l) for s, l in zip(starts, lens)]  # tokens in the cache (computed or cached) per sequence
+        deps: list[list[tuple[int, int]]] = [[] for _ in range(n)]  # (j, tokens j must have) per hit i
+        for i in range(n):
+            if starts[i] <= 0:
+                continue
+            pages = set(p for p in block_tables[i][:(starts[i] + block_size - 1) // block_size] if p >= 0)
+            for j in range(n):
+                if j != i and pages.intersection(block_tables[j]):
+                    deps[i].append((j, min(starts[i], lens[j])))
+        calls = []
+        while any(d < l for d, l in zip(done, lens)):
+            call: dict[int, tuple[int, int]] = {}
+            budget = max_tokens
+            added = True
+            while added and budget > 0 and len(call) < max_batch:  # later sequences may unblock earlier hits
+                added = False
+                for i in range(n):
+                    if i in call or done[i] >= lens[i] or budget == 0 or len(call) >= max_batch:
+                        continue
+                    if any(done[j] < need for j, need in deps[i]):
+                        continue
+                    q = min(lens[i] - done[i], budget)
+                    call[i] = (done[i], q)
+                    done[i] += q
+                    budget -= q
+                    added = True
+            assert call, "varlen prefill planner made no progress"
+            calls.append([(i, *call[i]) for i in sorted(call)])
+        return calls
+
+    def prefill_varlen(self, which: int, tokens: list[list[int]], block_tables: list[list[int]], starts: list[int],
+                       temps: list[float] | None = None, want_sample: bool = True, seed: int = 0):
+        """prefill_many through ssdk_forward_varlen: every call carries up to 256 tokens of up to max_batch sequences of
+        any lengths (plan_varlen_calls), prefix-cache hits included.  A sequence's first token is sampled by the call that
+        holds its last prompt token; calls where no prompt ends sample nothing.  Returns one token per sequence (None
+        without want_sample)."""
+        n = len(tokens)
+        temps = list(temps) if temps is not None else [0.0] * n
+        out: list[int | None] = [None] * n
+        for call in self.plan_varlen_calls([len(t) for t in tokens], starts, block_tables, self.block_size, 256,
+                                           self.max_batch):
+            ends = [pos + q == len(tokens[i]) for i, pos, q in call]
+            toks = self.forward_varlen(which, [tokens[i][pos:pos + q] for i, pos, q in call], [pos for _, pos, _ in call],
+                                       [block_tables[i] for i, _, _ in call], [temps[i] for i, _, _ in call],
+                                       want_sample=(want_sample and any(ends)), seed=seed)
+            for k, (i, _, _) in enumerate(call):
+                if ends[k] and toks is not None:
+                    out[i] = toks[k]
+        return out if want_sample else None
+
     def spec_step(self, ctx_len: list[int], recovery: list[int], bt_target, bt_draft, temps_t: list[float],
                   temps_q: list[float], seed: int = 0):
         """One sync speculative step.  Returns (speculations [B,K+1], n_accept [B], recovery [B]) as numpy."""
