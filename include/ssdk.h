@@ -124,12 +124,17 @@ int ssdk_finalize(ssdk_handle h, void* stream);
 /* ---- the hot path ---------------------------------------------------------- */
 
 /* One synchronous speculative-decoding step for `batch` sequences:
- *   K+1 draft forwards (speculator_sync.py:25-69) -> one (K+1)-token target
+ *   K draft forwards (speculator_sync.py:25-69) -> one (K+1)-token target
  *   forward (verifier.py:54-106) -> accept/reject + recovery (utils/verify.py:5-181),
  * enqueued as ONE call with no host control flow per token.
+ * The reference's K+1-th draft forward only writes the draft KV of the last draft token d_K.  It is not run here: when a
+ * step accepts all K drafts (out_n_accept[b] == K), d_K's draft KV (position ctx_len + K) is NOT written.  Pass d_K as
+ * pending[b] to the sequence's next step, whose first draft forward writes it; otherwise write it with a one-token
+ * draft forward (ssdk_forward_tokens, want_sample = 0) before anything else uses the draft cache.
  *  in : ctx_len[b]      tokens already in both KV caches (= seq.num_cached_tokens,
  *                       engine/step.py:101) — the recovery token sits at this position
  *       recovery[b]     seq.recovery_token_id (speculator_sync.py:38-45)
+ *       pending[b]      the token at ctx_len-1 when its draft KV is still to be written, else -1 (NULL: none)
  *       block_tables_*  [batch, max_blocks_per_seq] int32, -1 padded
  *                       (helpers/runner_helpers.py:110-121), covering ctx_len+K+1 slots
  *       temp_t/temp_q   per-sequence temperatures (verifier.py:83-90)
@@ -139,7 +144,7 @@ int ssdk_finalize(ssdk_handle h, void* stream);
  *       out_recovery[b]          = next recovery token
  * Host pointers; the call blocks until the results are on the host. */
 int ssdk_spec_step(ssdk_handle h, int batch,
-                   const int32_t* ctx_len, const int64_t* recovery,
+                   const int32_t* ctx_len, const int64_t* recovery, const int64_t* pending,
                    const int32_t* block_tables_target, const int32_t* block_tables_draft,
                    const float* temp_t, const float* temp_q,
                    uint64_t seed, uint64_t step_id,
@@ -147,9 +152,10 @@ int ssdk_spec_step(ssdk_handle h, int batch,
                    void* stream);
 
 /* Device-resident variant for measurement: same work, inputs already staged on the
- * device by a previous ssdk_spec_step_stage(); nothing crosses PCIe. */
+ * device by a previous ssdk_spec_step_stage(); nothing crosses PCIe.  The device carries
+ * the pending token from step to step; the last step's d_K draft KV stays unwritten. */
 int ssdk_spec_step_stage(ssdk_handle h, int batch,
-                         const int32_t* ctx_len, const int64_t* recovery,
+                         const int32_t* ctx_len, const int64_t* recovery, const int64_t* pending,
                          const int32_t* block_tables_target, const int32_t* block_tables_draft,
                          const float* temp_t, const float* temp_q,
                          uint64_t seed, uint64_t step_id, void* stream);

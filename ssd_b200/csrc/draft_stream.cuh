@@ -1,5 +1,13 @@
 // draft_stream.cuh — the whole speculate phase of a sync-SD step (SpeculatorSync.speculate, engine/speculator_sync.py:25-69:
-// K+1 single-token draft forwards + K samplings) as ONE persistent kernel, batch 1.
+// K single-token draft forwards + K samplings) as ONE persistent kernel, batch 1.
+//
+// The reference runs a K+1-th draft forward that only writes the KV of the last draft token d_K (speculator_sync.py:46-56).
+// Here that KV is written by the NEXT step instead: when the previous step accepted all K drafts, d_K sits at position
+// ctx0 - 1 without draft KV ("pending"), and forward 0 carries it as a second, earlier row (row 0) next to the recovery
+// token (row 1).  Both rows share every weight slot, so row 0 costs FMAs but no weight bytes.  Row 0 is computed with
+// exactly the arithmetic of a one-token forward (same x values, same per-warp dot products and summation order), stores
+// its K/V, and produces no logits; its attention units run before row 1's, one device-wide barrier apart, so row 1's
+// attention reads row 0's K/V from the cache.
 //
 // Why: the 1B draft streams 2.47 GB per forward, but the kernel-per-op path has nine kernel boundaries per layer, during
 // each of which HBM idles.  The weights
@@ -25,7 +33,8 @@
 //   E  down-proj rows
 // then final norm -> lm_head rows -> in-kernel sampling (greedy argmax over the bf16 logits, lowest index wins, or the
 // Philox exponential race of layers/sampler.py:27-34 — the SAME scores sample_kernel computes, so the tokens are identical)
-// -> the next forward starts inside the same launch.  The last forward of a step only writes KV (speculator_sync.py:52-56).
+// -> the next forward starts inside the same launch.  With skip_last_head the last forward only writes KV (the reference's
+// K+1-th forward, speculator_sync.py:52-56); the engine no longer launches that forward (see the top of this file).
 // Rounding points are the reference's (SURVEY §8a checklist 1-4): every linear output, the residual, the norm output, q/k
 // after RoPE and the attention output are rounded to bf16; accumulation is fp32.
 //
@@ -81,7 +90,33 @@ struct DsParams {
   unsigned* attn_ticket;         // [KV] arrival tickets of the split-KV units, zero between phases
   int n_slots;                   // ring depth (3 .. kDsMaxSlots)
   DsLayer layers[kDsMaxLayers];
+  const int64_t* pend_tok;       // [1] (may be null): >= 0: the token at position ctx0 - 1, whose KV forward 0 writes as row 0
+  __nv_bfloat16* vec_row0;       // row 0's vectors (ds_row0_vecs layout); read only when a token is pending
 };
+
+// vectors of row 0 of a two-row forward 0, carved from p.vec_row0 like the engine carves the row-1 vectors
+struct DsVecs {
+  __nv_bfloat16 *qkv, *attn, *o, *down, *resid0, *resid1, *act;
+  SSDK_DEVINL __nv_bfloat16* resid(int i) const { return i ? resid1 : resid0; }  // no indexed array: stays in registers
+};
+SSDK_DEVINL DsVecs ds_row0_vecs(const DsParams& p, int hd) {
+  DsVecs v{};
+  __nv_bfloat16* b = p.vec_row0;
+  if (!b) return v;
+  v.qkv = b; b += ((p.H + 2 * p.KV) * hd + 7) / 8 * 8;
+  v.attn = b; b += p.H * hd;
+  v.o = b; b += p.d;
+  v.down = b; b += p.d;
+  v.resid0 = b; b += p.d;
+  v.resid1 = b; b += p.d;
+  v.act = b;
+  return v;
+}
+// floats of the x region of shared memory: one row of every GEMV input, two rows of the norm outputs (d each)
+__host__ SSDK_DEVINL int ds_xs_floats(int d, int ffn, int q_width) {
+  const int a = 2 * d > ffn ? 2 * d : ffn;
+  return a > q_width ? a : q_width;
+}
 
 // consumer-only block barrier (the producer warp runs on its own)
 SSDK_DEVINL void ds_sync() {
@@ -292,17 +327,61 @@ SSDK_DEVINL float ds_score(const DsSample& s, float logit, int idx) {
   return logit * s.invT - __logf(e);
 }
 
+// row 0 of a two-row forward 0: its x (a norm output in shared memory, or an L2-resident vector) and its output
+struct DsRow0 {
+  const float* xs;
+  const __nv_bfloat16* xg;
+  __nv_bfloat16* y;
+};
+// row 0's dot product: ds_dot_seg's arithmetic, with x read step by step from shared memory (a second x slice held in
+// registers for the whole phase does not fit next to row 1's: the kernel is at its register limit, 168 per thread)
+SSDK_DEVINL float ds_dot_seg0(const uint8_t* wseg, int steps, int lane, const float* x0) {
+  const uint4* wp = reinterpret_cast<const uint4*>(wseg) + lane;
+  float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
+#pragma unroll 2
+  for (int j = 0; j < steps; ++j) {
+    const float4 u = *reinterpret_cast<const float4*>(x0 + j * 256 + lane * 8);
+    const float4 v = *reinterpret_cast<const float4*>(x0 + j * 256 + lane * 8 + 4);
+    const uint4 w = wp[j * 32];
+    float2 f = ds_bf2(w.x);
+    a0 = fmaf(f.x, u.x, a0); a1 = fmaf(f.y, u.y, a1);
+    f = ds_bf2(w.y);
+    a2 = fmaf(f.x, u.z, a2); a3 = fmaf(f.y, u.w, a3);
+    f = ds_bf2(w.z);
+    a0 = fmaf(f.x, v.x, a0); a1 = fmaf(f.y, v.y, a1);
+    f = ds_bf2(w.w);
+    a2 = fmaf(f.x, v.z, a2); a3 = fmaf(f.y, v.w, a3);
+  }
+  return warp_sum((a0 + a1) + (a2 + a3));
+}
+SSDK_DEVINL void ds_load_vec(const __nv_bfloat16* v, int n, float* xs);
+// row 0's x in shared memory: r.xs as is, or r.xg (an L2-resident vector of n elements) staged into xs once every warp
+// holds row 1's x slice in registers
+SSDK_DEVINL const float* ds_row0_x(const DsRow0& r, float* xs, int n) {
+  if (r.xs) return r.xs;
+  ds_sync();
+  ds_load_vec(r.xg, n, xs);
+  return xs;
+}
+
 // rows of a K <= 2048 matrix: y[row] = bf16(W[row] . x)   (HEAD: logits + the warp's running best score)
-template <bool HEAD>
-SSDK_DEVINL void ds_consume_plain(DsRing& ring, const DsGeom& g, const float* xs, __nv_bfloat16* y, DsSample* smp) {
+// TWO: the same for row 0 from the same slot (its dot product is the one-row arithmetic on its own x)
+template <bool HEAD, bool TWO = false>
+SSDK_DEVINL void ds_consume_plain(DsRing& ring, const DsGeom& g, float* xs, __nv_bfloat16* y, DsSample* smp,
+                                  const DsRow0& r0 = DsRow0{}) {
+  static_assert(!(HEAD && TWO), "row 0 has no lm_head");
   if ((int)blockIdx.x >= g.nj) return;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int steps = g.K >> 8;
   float xr[kDsMaxSteps][8];
   ds_load_x(xs, steps, lane, xr);
+  const float* x0 = nullptr;
+  if constexpr (TWO) x0 = ds_row0_x(r0, xs, g.K);
   for (int s = (int)blockIdx.x; s < g.nj; s += (int)gridDim.x) {
     const uint8_t* st = ds_acquire(ring, 0);
     const float acc = ds_dot_seg(st + (size_t)warp * g.K * 2, steps, lane, xr);
+    float acc0 = 0.f;
+    if constexpr (TWO) acc0 = ds_dot_seg0(st + (size_t)warp * g.K * 2, steps, lane, x0);
     ds_release(ring, 0, lane);
     ring.taken += 1u;
     const int row = s * 8 + warp;
@@ -310,6 +389,7 @@ SSDK_DEVINL void ds_consume_plain(DsRing& ring, const DsGeom& g, const float* xs
       const __nv_bfloat16 o = f2bf(acc);
       if (!HEAD) {
         y[row] = o;
+        if constexpr (TWO) r0.y[row] = f2bf(acc0);
       } else {
         if (y) y[row] = o;
         smp->best = argmax_better(smp->best, ArgMax{ds_score(*smp, bf2f(o), row), row});
@@ -318,46 +398,66 @@ SSDK_DEVINL void ds_consume_plain(DsRing& ring, const DsGeom& g, const float* xs
   }
 }
 // gate|up pairs: act[i] = bf16(silu(bf16 g_i) * bf16 u_i)   (layers/activation.py:11-14 on the bf16-rounded linear output)
-SSDK_DEVINL void ds_consume_pair(DsRing& ring, const DsGeom& g, const float* xs, __nv_bfloat16* act) {
+SSDK_DEVINL float ds_silu_mul(float gate, float up) {
+  gate = bf16_round(gate);
+  up = bf16_round(up);
+  return (gate / (1.0f + __expf(-gate))) * up;
+}
+template <bool TWO>
+SSDK_DEVINL void ds_consume_pair(DsRing& ring, const DsGeom& g, float* xs, __nv_bfloat16* act, const DsRow0& r0) {
   if ((int)blockIdx.x >= g.nj) return;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int steps = g.K >> 8;
   float xr[kDsMaxSteps][8];
   ds_load_x(xs, steps, lane, xr);
+  const float* x0 = nullptr;
+  if constexpr (TWO) x0 = ds_row0_x(r0, xs, g.K);
   for (int s = (int)blockIdx.x; s < g.nj; s += (int)gridDim.x) {
+    float gate0 = 0.f, up0 = 0.f;
     const uint8_t* sg = ds_acquire(ring, 0);
-    float gate = ds_dot_seg(sg + (size_t)warp * g.K * 2, steps, lane, xr);
+    const float gate = ds_dot_seg(sg + (size_t)warp * g.K * 2, steps, lane, xr);
+    if constexpr (TWO) gate0 = ds_dot_seg0(sg + (size_t)warp * g.K * 2, steps, lane, x0);
     ds_release(ring, 0, lane);
     const uint8_t* su = ds_acquire(ring, 1);
-    float up = ds_dot_seg(su + (size_t)warp * g.K * 2, steps, lane, xr);
+    const float up = ds_dot_seg(su + (size_t)warp * g.K * 2, steps, lane, xr);
+    if constexpr (TWO) up0 = ds_dot_seg0(su + (size_t)warp * g.K * 2, steps, lane, x0);
     ds_release(ring, 1, lane);
     ring.taken += 2u;
     const int i = s * 8 + warp;
     if (lane == 0 && i < g.rows) {
-      gate = bf16_round(gate);
-      up = bf16_round(up);
-      act[i] = f2bf((gate / (1.0f + __expf(-gate))) * up);
+      act[i] = f2bf(ds_silu_mul(gate, up));
+      if constexpr (TWO) r0.y[i] = f2bf(ds_silu_mul(gate0, up0));
     }
   }
 }
 // rows of a K > 2048 matrix: the warps split (row, K segment) units; partial sums meet in shared memory, summed in
-// segment order
-SSDK_DEVINL void ds_consume_split(DsRing& ring, const DsGeom& g, const float* xs, float* res, __nv_bfloat16* y) {
+// segment order.  res: [2 rows][2 buffers][kDsWarps]
+template <bool TWO>
+SSDK_DEVINL void ds_consume_split(DsRing& ring, const DsGeom& g, float* xs, float* res, __nv_bfloat16* y,
+                                  const DsRow0& r0) {
   if ((int)blockIdx.x >= g.nj) return;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int row_in_job = warp / g.segs, seg = warp - row_in_job * g.segs;
   const int seg_len = g.K / g.segs, steps = seg_len >> 8;
   float xr[kDsMaxSteps][8];
   ds_load_x(xs + seg * seg_len, steps, lane, xr);
+  const float* x0 = nullptr;
+  if constexpr (TWO) x0 = ds_row0_x(r0, xs, g.K);
   const size_t w_off = ((size_t)row_in_job * g.K + (size_t)seg * seg_len) * 2;
   unsigned it = 0;
   for (int s = (int)blockIdx.x; s < g.nj; s += (int)gridDim.x, ++it) {
     const uint8_t* st = ds_acquire(ring, 0);
     const float acc = ds_dot_seg(st + w_off, steps, lane, xr);
+    float acc0 = 0.f;
+    if constexpr (TWO) acc0 = ds_dot_seg0(st + w_off, steps, lane, x0 + seg * seg_len);
     ds_release(ring, 0, lane);
     ring.taken += 1u;
     float* rb = res + (it & 1u) * kDsWarps;  // double buffered: the readers of job i may still be busy while job i+1 is summed
-    if (lane == 0) rb[warp] = acc;
+    float* rb0 = rb + 2 * kDsWarps;
+    if (lane == 0) {
+      rb[warp] = acc;
+      if constexpr (TWO) rb0[warp] = acc0;
+    }
     ds_sync();
     if ((int)threadIdx.x < g.rpj) {
       const int row = s * g.rpj + (int)threadIdx.x;
@@ -365,13 +465,29 @@ SSDK_DEVINL void ds_consume_split(DsRing& ring, const DsGeom& g, const float* xs
         float v = 0.f;
         for (int q = 0; q < g.segs; ++q) v += rb[(int)threadIdx.x * g.segs + q];
         y[row] = f2bf(v);
+        if constexpr (TWO) {
+          float v0 = 0.f;
+          for (int q = 0; q < g.segs; ++q) v0 += rb0[(int)threadIdx.x * g.segs + q];
+          r0.y[row] = f2bf(v0);
+        }
       }
     }
   }
 }
-SSDK_DEVINL void ds_consume(DsRing& ring, const DsGeom& g, const float* xs, float* res, __nv_bfloat16* y) {
-  if (g.kind == DS_PLAIN) ds_consume_plain<false>(ring, g, xs, y, nullptr);
-  else ds_consume_split(ring, g, xs, res, y);
+// two: two rows (row 0 = r0)
+SSDK_DEVINL void ds_consume(DsRing& ring, const DsGeom& g, float* xs, float* res, __nv_bfloat16* y, bool two,
+                            const DsRow0& r0) {
+  if (g.kind == DS_PLAIN) {
+    if (two) ds_consume_plain<false, true>(ring, g, xs, y, nullptr, r0);
+    else ds_consume_plain<false>(ring, g, xs, y, nullptr);
+  } else {
+    if (two) ds_consume_split<true>(ring, g, xs, res, y, r0);
+    else ds_consume_split<false>(ring, g, xs, res, y, r0);
+  }
+}
+SSDK_DEVINL void ds_consume_gu(DsRing& ring, const DsGeom& g, float* xs, __nv_bfloat16* act, bool two, const DsRow0& r0) {
+  if (two) ds_consume_pair<true>(ring, g, xs, act, r0);
+  else ds_consume_pair<false>(ring, g, xs, act, r0);
 }
 
 SSDK_DEVINL float ds_block_sum(float v, float* red) {  // all consumer threads get the result
@@ -494,9 +610,10 @@ SSDK_DEVINL void ds_load_kv(const DsParams& p, const int* bt_s, const __nv_bfloa
     }
   }
 }
+// vqkv / vattn: the q|k|v input and the attention output of the row (row 1: p.vec_qkv / p.vec_attn)
 template <int HD, int GMAX, int TB>  // TB = tokens per warp iteration
-SSDK_DEVINL void ds_attention_unit(const DsParams& p, int layer, int h, int s, int ns, int ctx, float* sm, int* flag,
-                                   const int* bt_s) {
+SSDK_DEVINL void ds_attention_unit(const DsParams& p, const __nv_bfloat16* vqkv, __nv_bfloat16* vattn, int layer, int h,
+                                   int s, int ns, int ctx, float* sm, int* flag, const int* bt_s) {
   constexpr int HALF = HD / 2;
   constexpr int EPL = HD / 32;  // elements per lane in the dot layout (dims lane*EPL ..)
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -529,8 +646,8 @@ SSDK_DEVINL void ds_attention_unit(const DsParams& p, int layer, int h, int s, i
       const int i = lane + 32 * t;
       x1[t] = x2[t] = 0.f;
       if (i < HALF) {
-        const unsigned short a = __ldcg(reinterpret_cast<const unsigned short*>(p.vec_qkv + col0 + i));
-        const unsigned short b = __ldcg(reinterpret_cast<const unsigned short*>(p.vec_qkv + col0 + HALF + i));
+        const unsigned short a = __ldcg(reinterpret_cast<const unsigned short*>(vqkv + col0 + i));
+        const unsigned short b = __ldcg(reinterpret_cast<const unsigned short*>(vqkv + col0 + HALF + i));
         x1[t] = __bfloat162float(__ushort_as_bfloat16(a));
         x2[t] = __bfloat162float(__ushort_as_bfloat16(b));
         ss += x1[t] * x1[t] + x2[t] * x2[t];
@@ -662,7 +779,7 @@ SSDK_DEVINL void ds_attention_unit(const DsParams& p, int layer, int h, int s, i
       }
     }
     if (ns == 1) {  // the only split: this is the attention output
-      p.vec_attn[(size_t)(h * G + g) * HD + dim] = f2bf(ll > 0.f ? o / ll : 0.f);
+      vattn[(size_t)(h * G + g) * HD + dim] = f2bf(ll > 0.f ? o / ll : 0.f);
     } else {
       float* out = p.attn_part + ((size_t)(h * G + g) * kDsSplits + s) * LDR;
       out[dim] = o;  // un-normalised: sum_t 2^(s_t - mx) v_t
@@ -703,7 +820,7 @@ SSDK_DEVINL void ds_attention_unit(const DsParams& p, int layer, int h, int s, i
         o += os[q] * wt;
         l += ls[q] * wt;
       }
-      p.vec_attn[(size_t)(h * G + g) * HD + dim] = f2bf(l > 0.f ? o / l : 0.f);
+      vattn[(size_t)(h * G + g) * HD + dim] = f2bf(l > 0.f ? o / l : 0.f);
     }
   }
   ds_sync();
@@ -717,14 +834,14 @@ __global__ void __launch_bounds__(kDsThreads, 1) draft_stream_kernel(const __gri
   SSDK_STATIC_SMEM(uint64_t, empty_bar, kDsMaxSlots);
   SSDK_STATIC_SMEM(DsGeom, geom, 5);
   SSDK_STATIC_SMEM(float, red, 32);
-  SSDK_STATIC_SMEM(float, res, 2 * kDsWarps);
+  SSDK_STATIC_SMEM(float, res, 4 * kDsWarps);
   SSDK_STATIC_SMEM(ArgMax, ared, 32);
   SSDK_SHARED_VAR(int, tok_s);
   SSDK_SHARED_VAR(int, flag_s);
   SSDK_STATIC_SMEM(int, bt_s, kDsBtSmem);
-  // dynamic shared memory: [ring: n_slots x 32 KB][xs: max(d, ffn, H*HD) floats][attention scratch]
+  // dynamic shared memory: [ring: n_slots x 32 KB][xs: ds_xs_floats floats][attention scratch]
   float* xs = reinterpret_cast<float*>(ds_smem + (size_t)p.n_slots * kDsSlotBytes);
-  float* scratch = xs + max(max(p.d, p.ffn), p.H * HD);
+  float* scratch = xs + ds_xs_floats(p.d, p.ffn, p.H * HD);
   if (threadIdx.x < kDsBtSmem && (int)threadIdx.x < p.max_blocks) bt_s[threadIdx.x] = p.block_table[threadIdx.x];
   if (threadIdx.x == 0) {
     trace_mark(TR_MISC);
@@ -765,11 +882,15 @@ __global__ void __launch_bounds__(kDsThreads, 1) draft_stream_kernel(const __gri
   const uint64_t call0 = p.dyn ? p.dyn[1] * 16ull : p.call_base;
   __nv_bfloat16* resid[2] = {p.resid0, p.resid1};
   long long tok = p.tok_buf[0];
+  // a pending token: forward 0 also runs row 0 (that token at position ctx_base - 1; its x in xs[d, 2d) for the norms)
+  const long long tok0 = p.pend_tok ? p.pend_tok[0] : -1;
+  const DsVecs v0 = ds_row0_vecs(p, HD);
 
   for (int f = 0; f < p.n_fwd; ++f) {
     if (threadIdx.x == 0 && f > 0) trace_mark(TR_MISC);
     const int ctx = ctx_base + f + 1;  // tokens visible to this forward, the new one included
     const __nv_bfloat16* emb = p.embed + (size_t)tok * p.d;
+    const bool two = f == 0 && tok0 >= 0;
     int cur = 0;  // resid[cur] holds the residual entering the layer (layer 0: the embedding row itself)
     DsPre pre;    // operands of the next norm prologue, requested before the barrier in front of it
     for (int l = 0; l < p.L; ++l) {
@@ -777,13 +898,16 @@ __global__ void __launch_bounds__(kDsThreads, 1) draft_stream_kernel(const __gri
       // ---- A: (add +) input norm -> q|k|v ----
       if (l == 0) {
         // first layer: hidden = norm(embed), residual = embed (models/llama3.py:192-193)
+        if (two) ds_norm_prologue(p.embed + (size_t)tok0 * p.d, nullptr, v0.resid(cur ^ 1), lw.in_norm, p.eps, p.d, xs + p.d, red,
+                                  nullptr);
         ds_norm_prologue(emb, nullptr, resid[cur ^ 1], lw.in_norm, p.eps, p.d, xs, red, nullptr);
       } else {
+        if (two) ds_norm_prologue(v0.down, v0.resid(cur), v0.resid(cur ^ 1), lw.in_norm, p.eps, p.d, xs + p.d, red, nullptr);
         ds_norm_prologue(p.vec_down, resid[cur], resid[cur ^ 1], lw.in_norm, p.eps, p.d, xs, red, &pre);
       }
       cur ^= 1;
       ds_mark(f, 0);
-      ds_consume(ring, geom[DS_QKV], xs, res, p.vec_qkv);
+      ds_consume(ring, geom[DS_QKV], xs, res, p.vec_qkv, two, DsRow0{xs + p.d, nullptr, v0.qkv});
       ds_mark(f, 1);
       bar.sync();
       ds_mark(f, 2);
@@ -792,32 +916,44 @@ __global__ void __launch_bounds__(kDsThreads, 1) draft_stream_kernel(const __gri
       ds_mark(f, 12);
 #endif
       // ---- B: RoPE + KV store + attention units (+ merge by the last split of each kv head) ----
+      if (two) {
+        // row 0 first: its K/V store must be visible (device-wide barrier) before row 1's units read position ctx_base - 1
+        const int ns0 = ds_num_splits(ctx - 1);
+        for (int u = blockIdx.x; u < p.KV * ns0; u += gridDim.x) {
+          if (ns0 == kDsSplits)
+            ds_attention_unit<HD, GMAX, 8>(p, v0.qkv, v0.attn, l, u / ns0, u % ns0, ns0, ctx - 1, scratch, &flag_s, bt_s);
+          else ds_attention_unit<HD, GMAX, 4>(p, v0.qkv, v0.attn, l, u / ns0, u % ns0, ns0, ctx - 1, scratch, &flag_s, bt_s);
+        }
+        bar.sync();
+      }
       const int ns = ds_num_splits(ctx);
       for (int u = blockIdx.x; u < p.KV * ns; u += gridDim.x) {
-        if (ns == kDsSplits) ds_attention_unit<HD, GMAX, 8>(p, l, u / ns, u % ns, ns, ctx, scratch, &flag_s, bt_s);
-        else ds_attention_unit<HD, GMAX, 4>(p, l, u / ns, u % ns, ns, ctx, scratch, &flag_s, bt_s);
+        if (ns == kDsSplits)
+          ds_attention_unit<HD, GMAX, 8>(p, p.vec_qkv, p.vec_attn, l, u / ns, u % ns, ns, ctx, scratch, &flag_s, bt_s);
+        else ds_attention_unit<HD, GMAX, 4>(p, p.vec_qkv, p.vec_attn, l, u / ns, u % ns, ns, ctx, scratch, &flag_s, bt_s);
       }
       ds_mark(f, 3);
       bar.sync();
       ds_mark(f, 4);
       // ---- C: o-proj ----
       ds_load_vec(p.vec_attn, p.H * HD, xs);
-      ds_consume(ring, geom[DS_O], xs, res, p.vec_o);
+      ds_consume(ring, geom[DS_O], xs, res, p.vec_o, two, DsRow0{nullptr, v0.attn, v0.o});
       ds_mark(f, 5);
       pre = ds_preload(resid[cur], lw.post_norm, p.d);
       bar.sync();
       ds_mark(f, 6);
       // ---- D: add + post-attention norm -> gate|up with SiLU*mul ----
+      if (two) ds_norm_prologue(v0.o, v0.resid(cur), v0.resid(cur ^ 1), lw.post_norm, p.eps, p.d, xs + p.d, red, nullptr);
       ds_norm_prologue(p.vec_o, resid[cur], resid[cur ^ 1], lw.post_norm, p.eps, p.d, xs, red, &pre);
       cur ^= 1;
       ds_mark(f, 7);
-      ds_consume_pair(ring, geom[DS_GU], xs, p.vec_act);
+      ds_consume_gu(ring, geom[DS_GU], xs, p.vec_act, two, DsRow0{xs + p.d, nullptr, v0.act});
       ds_mark(f, 8);
       bar.sync();
       ds_mark(f, 9);
       // ---- E: down-proj ----
       ds_load_vec(p.vec_act, p.ffn, xs);
-      ds_consume(ring, geom[DS_DOWN], xs, res, p.vec_down);
+      ds_consume(ring, geom[DS_DOWN], xs, res, p.vec_down, two, DsRow0{nullptr, v0.act, v0.down});
       ds_mark(f, 10);
       pre = ds_preload(resid[cur], l + 1 < p.L ? p.layers[l + 1].in_norm : p.final_norm, p.d);
       bar.sync();

@@ -105,9 +105,12 @@ SSDK_DEVINL void gemm_out_at2x2(const GemmOut& g, int m, int a, int b, float* fa
 // prep: positions / slot_mapping / context_lens for one forward of `batch` sequences
 // with q_len tokens each, token j of sequence b at position ctx0[b] + pos_offset + j.
 // Mirrors prepare_decode_tensors_from_seqs (helpers/runner_helpers.py:50-108) on device.
+// pend (may be null): token 0 of sequence b gets slot -1 (no K/V store) unless pend[b] >= 0 — the two-row first draft
+// forward of a spec step, whose row 0 writes the K/V of a pending token only.
 // ----------------------------------------------------------------------------------
 __global__ void prep_kernel(const int32_t* __restrict__ ctx0, const int32_t* __restrict__ block_tables,
                             int max_blocks, int block_size, int batch, int q_len, int pos_offset,
+                            const int64_t* __restrict__ pend,
                             int64_t* __restrict__ positions, int32_t* __restrict__ slot_mapping,
                             int32_t* __restrict__ context_lens, unsigned* __restrict__ fwd_seq) {
   pdl_launch_dependents();
@@ -119,7 +122,8 @@ __global__ void prep_kernel(const int32_t* __restrict__ ctx0, const int32_t* __r
     const int pos = ctx0[b] + pos_offset + j;
     positions[i] = pos;
     const int blk = block_tables[(size_t)b * max_blocks + pos / block_size];
-    slot_mapping[i] = (blk < 0) ? -1 : blk * block_size + pos % block_size;
+    const bool masked = pend && j == 0 && pend[b] < 0;
+    slot_mapping[i] = (blk < 0 || masked) ? -1 : blk * block_size + pos % block_size;
   }
   if (i < batch) context_lens[i] = ctx0[i] + pos_offset + q_len;
   if (fwd_seq && i == 0) *fwd_seq += 1u;  // epoch base of this forward's one-shot all-reduces (tensor parallel target)

@@ -261,7 +261,8 @@ struct Workspace {
   // step state
   uint8_t* out_dev;     // [tok_buf | n_accept | recovery] — one D2H per step
   int64_t* tok_buf;     // [max_batch, K+1]
-  int64_t* ids_in;      // [kMaxTokens]  (forward_tokens input), followed by the varlen inputs (kFwIn*)
+  int64_t* fold_ids;    // [max_batch, 2]: {token at ctx-1, recovery} — the kernel-per-op draft's two-row forward 0
+  int64_t* ids_in;     // [kMaxTokens]  (forward_tokens input), followed by the varlen inputs (kFwIn*)
   int32_t* var_cu_q;    // [kMaxTokens + 1]  (forward_varlen prefix sums of q_len)
   AttnTile* var_tiles;  // [kMaxTokens]      (forward_varlen attention tile table)
   int64_t* out_tok;     // [max_batch]   (forward_tokens sampled output)
@@ -283,6 +284,7 @@ struct Workspace {
   size_t partial_floats = 0;
   // streaming draft kernel (draft_stream.cuh): inter-phase vectors, split-KV partials, device-wide barrier state
   bf16* ds_vec;
+  bf16* ds_vec0;  // the same vectors for row 0 of a two-row forward 0
   float* ds_attn;
   unsigned* ds_sync;
 };
@@ -320,7 +322,7 @@ struct ssdk_engine {
   size_t step_bytes = 0;
   size_t out_bytes = 0;
   // offsets inside the step block
-  size_t off_ctx, off_rec, off_tt, off_tq, off_seed, off_btt, off_btd;
+  size_t off_ctx, off_rec, off_pend, off_tt, off_tq, off_seed, off_btt, off_btd;
   size_t off_out_nacc, off_out_rec;
   // graphs
   std::map<int, cudaGraphExec_t> spec_graphs;  // keyed by batch * 2 + (draft path: 1 = streaming kernel)
@@ -347,6 +349,9 @@ static void derive(Model& m) {
   m.qkv_dim = (m.H + 2 * m.KV) * m.hd;
   m.vocab_local = c.vocab / c.tp_size;
 }
+
+// elements of one row's inter-phase vectors of the streaming draft kernel (enqueue_draft_stream / ds_row0_vecs carve them)
+static size_t ds_vec_elems(int qkv, int d, int ffn, int q_width) { return (size_t)qkv + 4 * d + ffn + q_width + 64; }
 
 // workspace carve-up (pass base = nullptr to measure)
 static int64_t carve(ssdk_engine* e, uint8_t* base) {
@@ -420,7 +425,10 @@ static int64_t carve(ssdk_engine* e, uint8_t* base) {
   w.ver_rows = (RowPart*)take((size_t)kVerifyMaxRows * kVerifyCtas * sizeof(RowPart));
   w.ver_rec = (RecPart*)take((size_t)kVerifyMaxBatch * kVerifyCtas * sizeof(RecPart));
   w.ver_counters = (unsigned*)take(64);
-  w.ds_vec = (bf16*)take((size_t)(qmax + 4 * dmax + fmax + Hmax * hdmax + 64) * 2);
+  const size_t ds_elems = ds_vec_elems(qmax, dmax, fmax, Hmax * hdmax);
+  w.ds_vec = (bf16*)take(ds_elems * 2);
+  w.ds_vec0 = (bf16*)take(ds_elems * 2);
+  w.fold_ids = (int64_t*)take((size_t)MB * 2 * 8);
   w.ds_attn = (float*)take((size_t)Hmax * kDsSplits * (hdmax + 2) * 4);
   w.ds_sync = (unsigned*)take(256);
   return (int64_t)align_up(off, 1024);
@@ -448,6 +456,7 @@ struct Fwd {
   bf16* logits_out;
   int64_t logits_ld;
   const VarlenFwd* var = nullptr;  // set: B sequences of their own q_len packed into M rows (Q unused)
+  const int64_t* pend = nullptr;   // set: row 0 of sequence b stores no K/V unless pend[b] >= 0 (prep_kernel)
 };
 
 static int attn_plan_raw(int H, int KV, int B, int Q, int max_ctx, int* TQ, int* MT, int* nqt, int* nsplit) {
@@ -658,7 +667,7 @@ static int enqueue_forward(ssdk_engine* e, Launcher& L, const Fwd& f) {
              w.positions, w.slot_mapping, w.context_lens, fwd_seq));
     TQ = f.var->plan.TQ; MT = f.var->plan.MT; nqt = f.var->plan.n_qtiles; nsplit = f.var->plan.n_split;
   } else {
-    CKI(L.go(prep_kernel, dim3(1), dim3(kMaxTokens), 0, f.ctx0, f.block_tables, mb, bs, f.B, f.Q, f.pos_offset,
+    CKI(L.go(prep_kernel, dim3(1), dim3(kMaxTokens), 0, f.ctx0, f.block_tables, mb, bs, f.B, f.Q, f.pos_offset, f.pend,
              w.positions, w.slot_mapping, w.context_lens, fwd_seq));
     CKI(attn_plan(m, f.B, f.Q, &TQ, &MT, &nqt, &nsplit, e->max_ctx_hint));
   }
@@ -829,6 +838,7 @@ static void layout_step(ssdk_engine* e) {
   auto take = [&](size_t n) { size_t o = off; off = align_up(off + n, 16); return o; };
   e->off_ctx = take((size_t)MB * 4);
   e->off_rec = take((size_t)MB * 8);
+  e->off_pend = take((size_t)MB * 8);
   e->off_tt = take((size_t)MB * 4);
   e->off_tq = take((size_t)MB * 4);
   e->off_seed = take(16);
@@ -842,21 +852,29 @@ static void layout_step(ssdk_engine* e) {
 
 
 
-// copy the recovery tokens into column 0 of the speculation buffer (speculator_sync.py:38-45)
-__global__ void init_tokens_kernel(const int64_t* __restrict__ recovery, int64_t* __restrict__ tok_buf, int B, int Kp1) {
+// copy the recovery tokens into column 0 of the speculation buffer (speculator_sync.py:38-45), and the ids of the
+// kernel-per-op draft's two-row forward 0: {token at ctx-1 (the recovery token again when nothing is pending: computed,
+// never stored), recovery}
+__global__ void init_tokens_kernel(const int64_t* __restrict__ recovery, const int64_t* __restrict__ pend,
+                                   int64_t* __restrict__ tok_buf, int64_t* __restrict__ fold_ids, int B, int Kp1) {
   pdl_launch_dependents();
   pdl_wait();
   const int b = threadIdx.x;
-  if (b < B) tok_buf[(size_t)b * Kp1] = recovery[b];
+  if (b < B) {
+    tok_buf[(size_t)b * Kp1] = recovery[b];
+    fold_ids[2 * b] = pend[b] >= 0 ? pend[b] : recovery[b];
+    fold_ids[2 * b + 1] = recovery[b];
+  }
 }
 
 // Device-resident bookkeeping between two spec steps (resident mode only): what
 // Scheduler.postprocess_speculate does to num_cached_tokens / recovery_token_id
-// (engine/scheduler.py:248-262), plus an on-device log of the accepted tokens.
-__global__ void advance_kernel(int32_t* __restrict__ ctx, int64_t* __restrict__ recovery_in, uint64_t* __restrict__ seed_step,
-                               const int64_t* __restrict__ tok_buf, const int32_t* __restrict__ n_accept,
-                               const int64_t* __restrict__ recovery_out, int64_t* __restrict__ log_tokens,
-                               int32_t* __restrict__ log_len, int B, int Kp1, int log_cap) {
+// (engine/scheduler.py:248-262), plus an on-device log of the accepted tokens.  A step that accepted all K drafts leaves
+// the draft KV of d_K (position ctx-1 of the next step) to the next step's first draft forward: pend = d_K, else -1.
+__global__ void advance_kernel(int32_t* __restrict__ ctx, int64_t* __restrict__ recovery_in, int64_t* __restrict__ pend,
+                               uint64_t* __restrict__ seed_step, const int64_t* __restrict__ tok_buf,
+                               const int32_t* __restrict__ n_accept, const int64_t* __restrict__ recovery_out,
+                               int64_t* __restrict__ log_tokens, int32_t* __restrict__ log_len, int B, int Kp1, int log_cap) {
   pdl_launch_dependents();
   pdl_wait();
   const int b = threadIdx.x;
@@ -867,15 +885,19 @@ __global__ void advance_kernel(int32_t* __restrict__ ctx, int64_t* __restrict__ 
     log_len[b] = len;
     ctx[b] += n;
     recovery_in[b] = recovery_out[b];
+    pend[b] = (n == Kp1) ? tok_buf[(size_t)b * Kp1 + Kp1 - 1] : -1;
   }
   if (threadIdx.x == 0) seed_step[1] += 1;
 }
 
 // ------------------------------------------------------------------------------------------
-// spec step: K+1 draft forwards -> (K+1)-token target forward -> verify      (enqueue only)
+// spec step: K draft forwards -> (K+1)-token target forward -> verify      (enqueue only)
+// The reference's K+1-th draft forward (KV of d_K only) is folded into the next step's first draft forward as its row 0
+// when the step accepted all K drafts (pend[b] >= 0, the token at ctx-1); the host flushes it with a one-token draft
+// forward when the sequence does not continue (PairRunner).
 // ------------------------------------------------------------------------------------------
 // ------------------------------------------------------------------------------------------
-// streaming draft kernel: the K+1 draft forwards + K samplings of a step in ONE cooperative launch (draft_stream.cuh)
+// streaming draft kernel: the K draft forwards + K samplings of a step in ONE cooperative launch (draft_stream.cuh)
 // SSDK_DRAFT_STREAM=0 keeps the kernel-per-op path.
 // ------------------------------------------------------------------------------------------
 static bool draft_stream_enabled() {
@@ -886,7 +908,7 @@ static bool draft_stream_enabled() {
 constexpr int kMaxDynSmem = 227 * 1024 - 2048;  // opt-in limit per CTA minus the kernel's static shared memory (1.8 KB)
 static size_t ds_fixed_smem(const Model& m) {
   const int G = m.H / m.KV, gmax = G <= 4 ? 4 : 8;
-  const size_t xs = (size_t)std::max(std::max(m.d, m.ffn), m.H * m.hd);
+  const size_t xs = (size_t)ds_xs_floats(m.d, m.ffn, m.H * m.hd);
   const size_t scratch = (size_t)gmax * m.hd + 2 * m.hd + (size_t)kDsWarps * gmax * (m.hd + 2);
   return (xs + scratch) * 4 + 256;
 }
@@ -941,8 +963,9 @@ static int launch_draft_stream(Launcher& L, const DsParams& p, size_t smem) {
   ++L.count;
   return 0;
 }
-// forwards 0 .. n_fwd-1 of the draft on tok_buf[0 ..]; samples tok_buf[f + 1] after every forward but (optionally) the last
-static int enqueue_draft_stream(ssdk_engine* e, Launcher& L, int64_t* tok_buf, int n_fwd, bool skip_last_head,
+// forwards 0 .. n_fwd-1 of the draft on tok_buf[0 ..]; samples tok_buf[f + 1] after every forward; forward 0 also writes
+// the KV of pend[0] at ctx0 - 1 when pend[0] >= 0
+static int enqueue_draft_stream(ssdk_engine* e, Launcher& L, int64_t* tok_buf, int n_fwd, const int64_t* pend,
                                 const int32_t* ctx0, const int32_t* block_table, const float* temp, const uint64_t* dyn,
                                 bf16* logits, int64_t logits_ld) {
   Model& m = e->model[SSDK_DRAFT];
@@ -956,7 +979,8 @@ static int enqueue_draft_stream(ssdk_engine* e, Launcher& L, int64_t* tok_buf, i
   p.k_cache = m.k_cache; p.v_cache = m.v_cache;
   p.cache_layer_stride = (long long)m.num_blocks * e->rt.block_size * m.KV * m.hd;
   p.block_size = e->rt.block_size; p.max_blocks = e->rt.max_blocks_per_seq;
-  p.tok_buf = tok_buf; p.n_fwd = n_fwd; p.skip_last_head = skip_last_head ? 1 : 0;
+  p.tok_buf = tok_buf; p.n_fwd = n_fwd; p.skip_last_head = 0;
+  p.pend_tok = pend; p.vec_row0 = w.ds_vec0;
   p.ctx0 = ctx0; p.block_table = block_table;
   bf16* v = w.ds_vec;
   p.vec_qkv = v; v += align_up((size_t)m.qkv_dim, 8);
@@ -997,6 +1021,7 @@ static int enqueue_spec_step(ssdk_engine* e, Launcher& L, int B, bool host_io, b
   }
   int32_t* ctx = (int32_t*)(w.step_dev + e->off_ctx);
   int64_t* rec_in = (int64_t*)(w.step_dev + e->off_rec);
+  int64_t* pend = (int64_t*)(w.step_dev + e->off_pend);
   const float* tt = (const float*)(w.step_dev + e->off_tt);
   const float* tq = (const float*)(w.step_dev + e->off_tq);
   uint64_t* seed_step = (uint64_t*)(w.step_dev + e->off_seed);
@@ -1006,25 +1031,28 @@ static int enqueue_spec_step(ssdk_engine* e, Launcher& L, int B, bool host_io, b
   const int tp = tgt.cfg.tp_size, tp_rank = tgt.cfg.tp_rank;
   if (tp > 1 && !e->comm) return fail("tensor parallel spec step without a NCCL communicator");
   if (tp_rank == 0 && !drf.present) return fail("rank 0 needs the draft model");
-  if (drf.present) CKI(L.go(init_tokens_kernel, dim3(1), dim3(64), 0, (const int64_t*)rec_in, w.tok_buf, B, K + 1));
+  if (drf.present)
+    CKI(L.go(init_tokens_kernel, dim3(1), dim3(64), 0, (const int64_t*)rec_in, (const int64_t*)pend, w.tok_buf, w.fold_ids,
+             B, K + 1));
   if (stream_draft)
-    CKI(enqueue_draft_stream(e, L, w.tok_buf, K + 1, true, ctx, btd, tq, seed_step, w.logits_q, (int64_t)V));
-  for (int k = 0; k <= K && drf.present && !stream_draft; ++k) {
+    CKI(enqueue_draft_stream(e, L, w.tok_buf, K, pend, ctx, btd, tq, seed_step, w.logits_q, (int64_t)V));
+  for (int k = 0; k < K && drf.present && !stream_draft; ++k) {
     Fwd f;
     f.which = SSDK_DRAFT; f.B = B; f.Q = 1; f.ids = w.tok_buf + k; f.ids_stride = K + 1;
     f.ctx0 = ctx; f.block_tables = btd; f.pos_offset = k;
-    // the K+1-th draft forward only writes the K-th draft token's KV (speculator_sync.py:52-56)
-    f.logits_mode = (k < K) ? 1 : 0;
+    f.logits_mode = 1;
+    if (k == 0) {
+      // two rows per sequence: the token at ctx-1 (K/V stored only when pending) and the recovery token; logits of row 1
+      f.Q = 2; f.ids = w.fold_ids; f.ids_stride = 1; f.pos_offset = -1; f.logits_mode = 2; f.pend = pend;
+    }
     f.logits_out = w.logits_q + (size_t)k * V;
     f.logits_ld = (int64_t)K * V;
     CKI(enqueue_forward(e, L, f));
-    if (k < K) {
-      SampleParams sp;
-      sp.logits = w.logits_q + (size_t)k * V; sp.ld = (int64_t)K * V; sp.temps = tq; sp.V = drf.cfg.vocab;
-      sp.seed = 0; sp.call_id = 0; sp.out = w.tok_buf + k + 1; sp.out_stride = K + 1;
-      sp.partial = w.samp_partial; sp.counters = w.samp_counters; sp.dyn = seed_step; sp.sub = k;
-      CKI(L.go(sample_kernel, dim3(kSampleChunks, B), dim3(256), 0, sp));
-    }
+    SampleParams sp;
+    sp.logits = w.logits_q + (size_t)k * V; sp.ld = (int64_t)K * V; sp.temps = tq; sp.V = drf.cfg.vocab;
+    sp.seed = 0; sp.call_id = 0; sp.out = w.tok_buf + k + 1; sp.out_stride = K + 1;
+    sp.partial = w.samp_partial; sp.counters = w.samp_counters; sp.dyn = seed_step; sp.sub = k;
+    CKI(L.go(sample_kernel, dim3(kSampleChunks, B), dim3(256), 0, sp));
   }
   if (tp > 1) {
     // the draft is pinned to rank 0: ship its K tokens (+ recovery) to the other ranks device-side
@@ -1054,7 +1082,7 @@ static int enqueue_spec_step(ssdk_engine* e, Launcher& L, int B, bool host_io, b
     L.barrier_op();
   }
   if (advance) {
-    CKI(L.go(advance_kernel, dim3(1), dim3(64), 0, ctx, rec_in, seed_step, (const int64_t*)w.tok_buf,
+    CKI(L.go(advance_kernel, dim3(1), dim3(64), 0, ctx, rec_in, pend, seed_step, (const int64_t*)w.tok_buf,
              (const int32_t*)w.n_accept, (const int64_t*)w.recovery, w.log_tokens, w.log_len, B, K + 1, kLogCap));
   }
   if (host_io) {
@@ -1336,12 +1364,18 @@ int ssdk_finalize(ssdk_handle h, void* stream) {
   return 0;
 }
 
-static int fill_step(ssdk_handle h, int batch, const int32_t* ctx_len, const int64_t* recovery, const int32_t* btt,
-                     const int32_t* btd, const float* tt, const float* tq, uint64_t seed, uint64_t step_id) {
+static int fill_step(ssdk_handle h, int batch, const int32_t* ctx_len, const int64_t* recovery, const int64_t* pending,
+                     const int32_t* btt, const int32_t* btd, const float* tt, const float* tq, uint64_t seed,
+                     uint64_t step_id) {
   if (batch < 1 || batch > h->rt.max_batch) return fail("batch %d out of range", batch);
   const int mbk = h->rt.max_blocks_per_seq;
   memcpy(h->pin_in + h->off_ctx, ctx_len, (size_t)batch * 4);
   memcpy(h->pin_in + h->off_rec, recovery, (size_t)batch * 8);
+  int64_t* pend = (int64_t*)(h->pin_in + h->off_pend);
+  for (int b = 0; b < batch; ++b) {
+    pend[b] = pending ? pending[b] : -1;
+    if (pend[b] >= 0 && ctx_len[b] < 1) return fail("spec_step: sequence %d has a pending token but no context", b);
+  }
   memcpy(h->pin_in + h->off_tt, tt, (size_t)batch * 4);
   memcpy(h->pin_in + h->off_tq, tq, (size_t)batch * 4);
   uint64_t ss[2] = {seed, step_id};
@@ -1357,14 +1391,15 @@ static void read_step(ssdk_handle h, int batch, int64_t* out_tokens, int32_t* ou
   if (out_recovery) memcpy(out_recovery, h->pin_out + h->off_out_rec, (size_t)batch * 8);
 }
 
-int ssdk_spec_step(ssdk_handle h, int batch, const int32_t* ctx_len, const int64_t* recovery,
+int ssdk_spec_step(ssdk_handle h, int batch, const int32_t* ctx_len, const int64_t* recovery, const int64_t* pending,
                    const int32_t* block_tables_target, const int32_t* block_tables_draft, const float* temp_t,
                    const float* temp_q, uint64_t seed, uint64_t step_id, int64_t* out_tokens, int32_t* out_n_accept,
                    int64_t* out_recovery, void* stream) {
   if (!h || !h->finalized) return fail("spec_step: engine not finalized");
   if (h->rt.spec_k < 1) return fail("spec_step: engine built without speculation");
   cudaStream_t st = (cudaStream_t)stream;
-  CKI(fill_step(h, batch, ctx_len, recovery, block_tables_target, block_tables_draft, temp_t, temp_q, seed, step_id));
+  CKI(fill_step(h, batch, ctx_len, recovery, pending, block_tables_target, block_tables_draft, temp_t, temp_q, seed,
+                step_id));
   const bool stream_draft = use_draft_stream(h, batch, *std::max_element(ctx_len, ctx_len + batch));
   if (h->rt.use_graph) {
     cudaGraphExec_t g;
@@ -1384,12 +1419,13 @@ int ssdk_spec_step(ssdk_handle h, int batch, const int32_t* ctx_len, const int64
   return 0;
 }
 
-int ssdk_spec_step_stage(ssdk_handle h, int batch, const int32_t* ctx_len, const int64_t* recovery,
+int ssdk_spec_step_stage(ssdk_handle h, int batch, const int32_t* ctx_len, const int64_t* recovery, const int64_t* pending,
                          const int32_t* block_tables_target, const int32_t* block_tables_draft, const float* temp_t,
                          const float* temp_q, uint64_t seed, uint64_t step_id, void* stream) {
   if (!h || !h->finalized) return fail("spec_step_stage: engine not finalized");
   cudaStream_t st = (cudaStream_t)stream;
-  CKI(fill_step(h, batch, ctx_len, recovery, block_tables_target, block_tables_draft, temp_t, temp_q, seed, step_id));
+  CKI(fill_step(h, batch, ctx_len, recovery, pending, block_tables_target, block_tables_draft, temp_t, temp_q, seed,
+                step_id));
   h->resident_ctx_bound = *std::max_element(ctx_len, ctx_len + batch);
   CK(cudaMemcpyAsync(h->ws.step_dev, h->pin_in, h->step_bytes, cudaMemcpyHostToDevice, st));
   CK(cudaMemsetAsync(h->ws.log_len, 0, (size_t)h->rt.max_batch * 4, st));

@@ -56,9 +56,9 @@ SIGNATURES: dict[str, tuple] = {
     "ssdk_symm_bytes": (C.c_int64, [VP]),
     "ssdk_bind_symm": (C.c_int, [VP, C.POINTER(VP), C.c_int]),
     "ssdk_finalize": (C.c_int, [VP, VP]),
-    "ssdk_spec_step": (C.c_int, [VP, C.c_int, c_i32p, c_i64p, c_i32p, c_i32p, c_f32p, c_f32p, C.c_uint64, C.c_uint64,
-                                 c_i64p, c_i32p, c_i64p, VP]),
-    "ssdk_spec_step_stage": (C.c_int, [VP, C.c_int, c_i32p, c_i64p, c_i32p, c_i32p, c_f32p, c_f32p, C.c_uint64,
+    "ssdk_spec_step": (C.c_int, [VP, C.c_int, c_i32p, c_i64p, c_i64p, c_i32p, c_i32p, c_f32p, c_f32p, C.c_uint64,
+                                 C.c_uint64, c_i64p, c_i32p, c_i64p, VP]),
+    "ssdk_spec_step_stage": (C.c_int, [VP, C.c_int, c_i32p, c_i64p, c_i64p, c_i32p, c_i32p, c_f32p, c_f32p, C.c_uint64,
                                        C.c_uint64, VP]),
     "ssdk_spec_step_resident": (C.c_int, [VP, C.c_int, VP]),
     "ssdk_spec_step_fetch": (C.c_int, [VP, C.c_int, c_i64p, c_i32p, c_i64p, VP]),

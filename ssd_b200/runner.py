@@ -116,6 +116,11 @@ class PairRunner:
         L.check(self.lib.ssdk_bind_workspace(self.h, self.workspace.data_ptr() + off, nbytes), "ssdk_bind_workspace")
         self.finalized = False
         self.step_id = 0
+        # Draft KV the engine has not written yet: a spec step that accepts all K drafts leaves the KV of the last one,
+        # d_K, to the first draft forward of the sequence's next step (ssdk_spec_step).  One record per such row:
+        # (position, token, draft block table up to that position's page).  A spec step that continues the row folds it
+        # in; anything else that uses the draft cache first writes it with a one-token draft forward (flush_draft).
+        self._pending: list[tuple[int, int, tuple[int, ...]]] = []
 
     # ------------------------------------------------------------------ weights
     def bind_weights(self, which: int, w: dict) -> None:
@@ -165,6 +170,8 @@ class PairRunner:
         """ModelRunner.run for q_len tokens per sequence appended at ctx_len (prefill chunk or AR decode)."""
         if self.spec[which] is None:
             return None  # the draft replica lives on TP rank 0 only (SURVEY §8e); other ranks have nothing to do
+        if which == L.DRAFT:
+            self.flush_draft()
         B, Q = len(ids), len(ids[0])
         assert all(len(x) == Q for x in ids)
         ids_a = np.ascontiguousarray(np.array(ids, dtype=np.int64).reshape(-1))
@@ -250,6 +257,8 @@ class PairRunner:
         ctx_len[b]; with want_sample, the last row of every sequence is sampled."""
         if self.spec[which] is None:
             return None
+        if which == L.DRAFT:
+            self.flush_draft()
         B = len(ids)
         q_a = _i32([len(x) for x in ids])
         ids_a = np.ascontiguousarray(np.fromiter((t for x in ids for t in x), dtype=np.int64, count=int(q_a.sum())))
@@ -331,8 +340,21 @@ class PairRunner:
 
     def spec_step(self, ctx_len: list[int], recovery: list[int], bt_target, bt_draft, temps_t: list[float],
                   temps_q: list[float], seed: int = 0):
-        """One sync speculative step.  Returns (speculations [B,K+1], n_accept [B], recovery [B]) as numpy."""
+        """One sync speculative step.  Returns (speculations [B,K+1], n_accept [B], recovery [B]) as numpy.
+        A row that continues a row of an earlier step whose drafts were all accepted (same draft pages, ctx_len one past
+        the pending position) writes that step's d_K draft KV in its first draft forward; other pending rows are flushed
+        first."""
         B, K = len(ctx_len), self.K
+        pend = np.full(B, -1, dtype=np.int64)
+        rest = list(self._pending)
+        for b in range(B):
+            for i, (pos, tok, pages) in enumerate(rest):
+                if ctx_len[b] == pos + 1 and tuple(bt_draft[b][:len(pages)]) == pages:
+                    pend[b] = tok
+                    del rest[i]
+                    break
+        self._pending = rest
+        self.flush_draft()
         ctx_a, rec_a = _i32(ctx_len), np.ascontiguousarray(recovery, dtype=np.int64)
         btt, btd = self._bt(bt_target), self._bt(bt_draft)
         tt, tq = np.ascontiguousarray(temps_t, dtype=np.float32), np.ascontiguousarray(temps_q, dtype=np.float32)
@@ -341,22 +363,48 @@ class PairRunner:
         rec = np.zeros(B, dtype=np.int64)
         st = torch.cuda.current_stream().cuda_stream
         L.check(self.lib.ssdk_spec_step(self.h, B, ctx_a.ctypes.data_as(L.c_i32p), rec_a.ctypes.data_as(L.c_i64p),
-                                        btt.ctypes.data_as(L.c_i32p), btd.ctypes.data_as(L.c_i32p),
-                                        tt.ctypes.data_as(L.c_f32p), tq.ctypes.data_as(L.c_f32p), seed, self.step_id,
-                                        toks.ctypes.data_as(L.c_i64p), nacc.ctypes.data_as(L.c_i32p),
-                                        rec.ctypes.data_as(L.c_i64p), st), "ssdk_spec_step")
+                                        pend.ctypes.data_as(L.c_i64p), btt.ctypes.data_as(L.c_i32p),
+                                        btd.ctypes.data_as(L.c_i32p), tt.ctypes.data_as(L.c_f32p),
+                                        tq.ctypes.data_as(L.c_f32p), seed, self.step_id, toks.ctypes.data_as(L.c_i64p),
+                                        nacc.ctypes.data_as(L.c_i32p), rec.ctypes.data_as(L.c_i64p), st), "ssdk_spec_step")
         self.step_id += 1
+        if self.spec[L.DRAFT] is not None:
+            for b in range(B):
+                if int(nacc[b]) == K:
+                    pos = ctx_len[b] + K
+                    self._pending.append((pos, int(toks[b, K]), tuple(bt_draft[b][:pos // self.block_size + 1])))
         return toks, nacc, rec
 
-    # resident (device-driven) mode used by bench.py's kernel-only measurement
+    def flush_draft(self) -> None:
+        """Write the draft KV that spec steps left pending (one one-token, headless draft forward for all of them).
+        Runs before any other use of the draft cache; call it before reading self.kv[DRAFT] directly."""
+        if not self._pending or self.spec[L.DRAFT] is None:
+            self._pending = []
+            return
+        recs, self._pending = self._pending, []
+        B = len(recs)
+        ids_a = np.ascontiguousarray([tok for _, tok, _ in recs], dtype=np.int64)
+        ctx_a, bt_a = _i32([pos for pos, _, _ in recs]), self._bt([list(pages) for _, _, pages in recs])
+        temps_a = np.zeros(B, dtype=np.float32)
+        out = np.zeros(B, dtype=np.int64)
+        # step_id is not advanced: the Philox streams of later calls stay those of a run without the deferral
+        L.check(self.lib.ssdk_forward_tokens(self.h, L.DRAFT, B, 1, ids_a.ctypes.data_as(L.c_i64p),
+                                             ctx_a.ctypes.data_as(L.c_i32p), bt_a.ctypes.data_as(L.c_i32p), 0,
+                                             temps_a.ctypes.data_as(L.c_f32p), 0, self.step_id,
+                                             out.ctypes.data_as(L.c_i64p), torch.cuda.current_stream().cuda_stream),
+                "ssdk_forward_tokens (draft flush)")
+
+    # resident (device-driven) mode used by bench.py's kernel-only measurement.  The device carries the pending d_K from
+    # step to step; the last resident step's one stays unwritten.
     def stage(self, ctx_len, recovery, bt_target, bt_draft, temps_t, temps_q, seed: int = 0):
+        self.flush_draft()
         B = len(ctx_len)
         ctx_a, rec_a = _i32(ctx_len), np.ascontiguousarray(recovery, dtype=np.int64)
         btt, btd = self._bt(bt_target), self._bt(bt_draft)
         tt, tq = np.ascontiguousarray(temps_t, dtype=np.float32), np.ascontiguousarray(temps_q, dtype=np.float32)
         st = torch.cuda.current_stream().cuda_stream
         L.check(self.lib.ssdk_spec_step_stage(self.h, B, ctx_a.ctypes.data_as(L.c_i32p), rec_a.ctypes.data_as(L.c_i64p),
-                                              btt.ctypes.data_as(L.c_i32p), btd.ctypes.data_as(L.c_i32p),
+                                              None, btt.ctypes.data_as(L.c_i32p), btd.ctypes.data_as(L.c_i32p),
                                               tt.ctypes.data_as(L.c_f32p), tq.ctypes.data_as(L.c_f32p), seed,
                                               self.step_id, st), "ssdk_spec_step_stage")
 
@@ -397,7 +445,7 @@ class PairRunner:
         (layout_step() in csrc/engine.cu; every field 16-byte aligned)."""
         a = lambda n: (n + 15) // 16 * 16
         MB, mbk, K = self.max_batch, self.max_blocks, self.K
-        h2d = a(MB * 4) + a(MB * 8) + 2 * a(MB * 4) + 16 + 2 * a(MB * mbk * 4)
+        h2d = a(MB * 4) + 2 * a(MB * 8) + 2 * a(MB * 4) + 16 + 2 * a(MB * mbk * 4)
         d2h = a(a(MB * (K + 1) * 8) + a(MB * 4) + MB * 8)
         return h2d, d2h
 

@@ -1,4 +1,4 @@
-"""Validate the streaming draft kernel (csrc/draft_stream.cuh, one persistent launch per step for the K+1 draft forwards
+"""Validate the streaming draft kernel (csrc/draft_stream.cuh, one persistent launch per step for the K draft forwards
 and their samplings) against the kernel-per-op path (SSDK_DRAFT_STREAM=0).
 
     python tools/check_draft_stream.py [--temp 0.7] [--prompt-len 3000] [--parallel]
