@@ -98,6 +98,19 @@ int ssdk_destroy(ssdk_handle h);
 int ssdk_bind_weight(ssdk_handle h, int which, int kind, int layer,
                      const void* dev_ptr, int64_t rows, int64_t cols);
 
+/* FP8 weight-only (W8A16) form of a target decoder linear.  The reference has
+ * no FP8 path.  kind: SSDK_W_QKV, SSDK_W_O, SSDK_W_GATE_UP or SSDK_W_DOWN;
+ * which: SSDK_TARGET only (the draft stays bf16).  Layout, no packing step:
+ *   w_e4m3    float8 e4m3fn [rows, cols] row-major, same shape and row order as
+ *             the bf16 matrix of that kind (q|k|v and gate|up packed), 16-byte aligned;
+ *   row_scale fp32 [rows]: row n of the matrix is row_scale[n] * W8[n, :].
+ * cols (K) must be a multiple of 128.  Both buffers stay owned by the caller
+ * and must outlive the handle.  The GEMM computes
+ *   y[m, n] = bf16( s[n] * sum_k bf16(W8[n, k]) * x[m, k] )   (fp32 accumulate). */
+int ssdk_bind_weight_fp8(ssdk_handle h, int which, int kind, int layer,
+                         const void* w_e4m3, const float* row_scale,
+                         int64_t rows, int64_t cols);
+
 /* Replaces ModelRunner.allocate_kv_cache (engine/model_runner.py:446-503):
  * one tensor [2, L, num_blocks, block_size, kv_heads/tp, hd] (bf16);
  * k = base, v = base + L*num_blocks*block_size*kv_heads/tp*hd elements. */
@@ -223,6 +236,21 @@ int ssdk_gemm_small_m(const void* x, const void* w, void* y, float* partials,
  * (layers/linear.py:101-122 + layers/activation.py:11-14), fused epilogue. */
 int ssdk_gemm_gate_up_silu(const void* x, const void* w_gate_up, void* h,
                            int M, int ffn, int K, void* stream);
+
+/* FP8-weight (e4m3 + fp32 per-row scale, layout of ssdk_bind_weight_fp8)
+ * versions of the two GEMMs above; the reference has no FP8 path.  M <= 256,
+ * K a multiple of 128.  The scale multiplies the fp32 accumulator before any
+ * rounding; split-K partials are stored scaled.  gate_up_silu_fp8: split_k <= 1
+ * runs one split; split_k > 1 (M <= 64) reduces inside the kernel and needs
+ * fp32 partials [split_k, M, 2*ffn] and ceil(ffn/64) zeroed uint32 counters
+ * (left zeroed on return). */
+int ssdk_gemm_small_m_fp8(const void* x, const void* w8, const float* scale,
+                          void* y, float* partials, int M, int N, int K,
+                          int ldy, int split_k, void* stream);
+int ssdk_gemm_gate_up_silu_fp8(const void* x, const void* w8_gate_up,
+                               const float* scale, void* h, float* partials,
+                               unsigned* counters, int M, int ffn, int K,
+                               int split_k, void* stream);
 
 /* RMSDNorm (layers/layernorm.py:53-98), compiled single-rounding semantics:
  * r = x (+ residual); residual_out = bf16(r); y = bf16(r * rsqrt(mean r^2 + eps) * w).

@@ -8,6 +8,7 @@ import os
 from dataclasses import dataclass
 
 from .paths import DEFAULT_DRAFT, DEFAULT_TARGET
+from .quant import checkpoint_quantization, parse_quantization
 
 
 @dataclass
@@ -49,6 +50,10 @@ class Config:
     # prefill through ssdk_forward_varlen (PairRunner.prefill_varlen): prompts of any lengths and prefix-cache hits share
     # 256-token calls.  Opt-in until measured on the H100 (DESIGN.md §7).
     varlen_prefill: bool = False
+    # "fp8": the target's four decoder linears (qkv, o, gate_up, down) run as e4m3 weights with fp32 per-row scales
+    # (W8A16, DESIGN.md §3); bf16 checkpoints are quantized on load.  This changes the outputs.  An FP8 checkpoint is
+    # loaded as FP8 whatever this says, and the field then reads "fp8".
+    quantization: str | None = None
 
     @property
     def max_blocks(self) -> int:
@@ -65,12 +70,18 @@ class Config:
             raise NotImplementedError("EAGLE-3 drafts are out of scope of the sync-SD hot path")
         if self.enforce_eager:
             self.use_cuda_graph = False
+        self.quantization = parse_quantization(self.quantization)
         self.hf_config = load_hf_config(self.model)
+        if checkpoint_quantization(self.hf_config) == "fp8":
+            self.quantization = "fp8"
         self.max_model_len = min(self.max_model_len, self.hf_config.max_position_embeddings)
         if self.speculate:
             if not os.path.isdir(self.draft):
                 raise AssertionError(f"draft directory {self.draft!r} does not exist")
             self.draft_hf_config = load_hf_config(self.draft)
+            if getattr(self.draft_hf_config, "quantization_config", None):
+                raise NotImplementedError(f"{self.draft}: quantized draft checkpoints are not supported (the draft runs "
+                                          "in bf16)")
             self.max_model_len = min(self.max_model_len, self.draft_hf_config.max_position_embeddings)
         if self.max_num_batched_tokens < self.max_model_len:
             raise AssertionError("max_num_batched_tokens < max_model_len (config.py:94)")

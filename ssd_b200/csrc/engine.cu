@@ -120,6 +120,22 @@ static int make_tmap(CUtensorMap* tm, const void* ptr, int64_t rows, int64_t col
                                      (long long)rows, (long long)cols, box_rows);
   return 0;
 }
+// e4m3 row-major [rows, cols] weight as bytes, box = [64 rows, 128 cols (= one 128 B swizzle row)], 128B swizzle
+static int make_tmap_e4m3(CUtensorMap* tm, const void* ptr, int64_t rows, int64_t cols) {
+  CKI(get_encode());
+  if (cols % kBlockK8 != 0) return fail("FP8 weight: K=%lld not a multiple of %d", (long long)cols, kBlockK8);
+  if (((uintptr_t)ptr & 15) != 0) return fail("TMA: base pointer not 16-byte aligned");
+  cuuint64_t gdim[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
+  cuuint64_t gstride[1] = {(cuuint64_t)cols};
+  cuuint32_t box[2] = {(cuuint32_t)kBlockK8, 64u};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = g_encode(tm, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void*>(ptr), gdim, gstride, box, estr,
+                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) return fail("cuTensorMapEncodeTiled (e4m3) failed (%d) rows=%lld cols=%lld", (int)r,
+                                     (long long)rows, (long long)cols);
+  return 0;
+}
 
 // ------------------------------------------------------------------------------------------
 // GEMM planning + launch
@@ -166,21 +182,25 @@ static int auto_splits(int tiles, int num_kb, int ctas_per_sm = 2) {
   return (num_kb + per - 1) / per;
 }
 
-template <int UN, int EPI>
+template <int UN, int EPI, bool FP8>
 static int launch_gemm_inst(Launcher& L, const CUtensorMap& tmW, const CUtensorMap& tmX, const GemmParams& p, int tiles,
-                            int splits) {
-  using Cfg = GemmCfg<UN>;
+                            int splits, const float* fp8_scale) {
+  using Cfg = GemmCfg<UN, FP8>;
   static bool attr_set = false;
   if (!attr_set) {
-    CK(cudaFuncSetAttribute(gemm_ws_kernel<UN, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+    CK(cudaFuncSetAttribute(gemm_ws_kernel<UN, EPI, FP8>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
     attr_set = true;
   }
-  return L.go(gemm_ws_kernel<UN, EPI>, dim3(tiles, splits), dim3(kGemmThreads), (size_t)Cfg::kSmemBytes, tmW, tmX, p);
+  return L.go(gemm_ws_kernel<UN, EPI, FP8>, dim3(tiles, splits), dim3(kGemmThreads), (size_t)Cfg::kSmemBytes, tmW, tmX, p,
+              fp8_scale);
 }
+// fp8_scale != nullptr: tmW is an e4m3 byte map (make_tmap_e4m3) and p.num_kb counts 128-k blocks
 static int launch_gemm(Launcher& L, int umma_n, int epi, const CUtensorMap& tmW, const CUtensorMap& tmX,
-                       const GemmParams& p, int tiles, int splits) {
-#define SSDK_GEMM_CASE(UN, EP) \
-  if (umma_n == UN && epi == EP) return launch_gemm_inst<UN, EP>(L, tmW, tmX, p, tiles, splits);
+                       const GemmParams& p, int tiles, int splits, const float* fp8_scale = nullptr) {
+#define SSDK_GEMM_CASE(UN, EP)                                                                                       \
+  if (umma_n == UN && epi == EP)                                                                                     \
+    return fp8_scale ? launch_gemm_inst<UN, EP, true>(L, tmW, tmX, p, tiles, splits, fp8_scale)                      \
+                     : launch_gemm_inst<UN, EP, false>(L, tmW, tmX, p, tiles, splits, nullptr);
   SSDK_GEMM_CASE(16, EPI_BF16) SSDK_GEMM_CASE(16, EPI_PARTIAL) SSDK_GEMM_CASE(16, EPI_SILU) SSDK_GEMM_CASE(16, EPI_PUBLISH)
   SSDK_GEMM_CASE(32, EPI_BF16) SSDK_GEMM_CASE(32, EPI_PARTIAL) SSDK_GEMM_CASE(32, EPI_SILU) SSDK_GEMM_CASE(32, EPI_PUBLISH)
   SSDK_GEMM_CASE(64, EPI_BF16) SSDK_GEMM_CASE(64, EPI_PARTIAL) SSDK_GEMM_CASE(64, EPI_SILU) SSDK_GEMM_CASE(64, EPI_PUBLISH)
@@ -191,7 +211,8 @@ static int launch_gemm(Launcher& L, int umma_n, int epi, const CUtensorMap& tmW,
 }
 
 struct WeightMat {
-  const bf16* ptr = nullptr;
+  const bf16* ptr = nullptr;  // bf16 [rows, cols]; with `scale` set: e4m3 bytes [rows, cols] (ssdk_bind_weight_fp8)
+  const float* scale = nullptr;  // fp32 [rows] per-row scales of an FP8 matrix, nullptr for bf16
   int64_t rows = 0, cols = 0;
   CUtensorMap tm;
   bool has_tm = false;
@@ -199,7 +220,8 @@ struct WeightMat {
 static int weight_tmap(WeightMat& w) {
   if (w.has_tm) return 0;
   if (!w.ptr) return fail("weight not bound");
-  CKI(make_tmap(&w.tm, w.ptr, w.rows, w.cols, 64));
+  if (w.scale) CKI(make_tmap_e4m3(&w.tm, w.ptr, w.rows, w.cols));
+  else CKI(make_tmap(&w.tm, w.ptr, w.rows, w.cols, 64));
   w.has_tm = true;
   return 0;
 }
@@ -376,7 +398,7 @@ static int64_t carve(ssdk_engine* e, uint8_t* base) {
     // partial buffer: max over GEMMs of S*M*N with S bounded by auto_splits (<= 2*SMs/tiles + 1)
     auto need = [&](int N, int K) {
       const int tiles = (N + kTileRows - 1) / kTileRows;
-      const int S = auto_splits(tiles, K / kBlockK);
+      const int S = std::max(auto_splits(tiles, K / kBlockK), auto_splits(tiles, std::max(1, K / kBlockK8)));  // bf16 / FP8
       return (size_t)S * kMaxTokens * N;
     };
     part = std::max(part, need(m.qkv_dim, m.d));
@@ -523,12 +545,13 @@ static int enqueue_gemm(ssdk_engine* e, Launcher& L, const bf16* x, WeightMat& w
                         int N_out, int* splits_out, const PublishParams* pub = nullptr) {
   CKI(weight_tmap(w));
   const int K = (int)w.cols;
-  if (K % kBlockK) return fail("GEMM K=%d not a multiple of 64", K);
+  const int kbk = w.scale ? kBlockK8 : kBlockK;  // an FP8 stage holds 128 k (bytes) of weights, a bf16 one 64 k
+  if (K % kbk) return fail("GEMM K=%d not a multiple of %d", K, kbk);
   const int un = umma_n_for(M);
   const CUtensorMap* tmX;
   CKI(e->xmaps.get(x, K, un, &tmX));
   GemmParams p;
-  p.out = out; p.M = M; p.N = N_out; p.ldo = ldo; p.num_kb = K / kBlockK;
+  p.out = out; p.M = M; p.N = N_out; p.ldo = ldo; p.num_kb = K / kbk;
   int tiles, splits;
   p.sk_partials = nullptr; p.sk_counters = nullptr; p.sk_width = 0;
   if (epi == EPI_SILU) {
@@ -559,7 +582,7 @@ static int enqueue_gemm(ssdk_engine* e, Launcher& L, const bf16* x, WeightMat& w
   if (epi == EPI_PARTIAL && (size_t)splits * M * N_out > e->ws.partial_floats && out == e->ws.partials)
     return fail("split-K partial buffer too small");
   if (splits_out) *splits_out = splits;
-  return launch_gemm(L, un, epi, w.tm, *tmX, p, tiles, splits);
+  return launch_gemm(L, un, epi, w.tm, *tmX, p, tiles, splits, w.scale);
 }
 
 // y = allreduce_sum(bf16(sum_s partials)) for tensor-parallel row-parallel linears
@@ -1129,8 +1152,11 @@ static int get_spec_graph(ssdk_engine* e, int B, bool host_io, bool stream_draft
 
 // pre-set >48 KB dynamic smem opt-ins so nothing but launches happens during capture
 static int init_kernel_attrs() {
-#define SSDK_ATTR_G(UN, EP) \
-  CK(cudaFuncSetAttribute(gemm_ws_kernel<UN, EP>, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmCfg<UN>::kSmemBytes));
+#define SSDK_ATTR_G(UN, EP)                                                                                    \
+  CK(cudaFuncSetAttribute(gemm_ws_kernel<UN, EP, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,          \
+                          GemmCfg<UN>::kSmemBytes));                                                           \
+  CK(cudaFuncSetAttribute(gemm_ws_kernel<UN, EP, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,           \
+                          GemmCfg<UN, true>::kSmemBytes));
   SSDK_ATTR_G(16, EPI_BF16) SSDK_ATTR_G(16, EPI_PARTIAL) SSDK_ATTR_G(16, EPI_SILU) SSDK_ATTR_G(16, EPI_PUBLISH)
   SSDK_ATTR_G(32, EPI_BF16) SSDK_ATTR_G(32, EPI_PARTIAL) SSDK_ATTR_G(32, EPI_SILU) SSDK_ATTR_G(32, EPI_PUBLISH)
   SSDK_ATTR_G(64, EPI_BF16) SSDK_ATTR_G(64, EPI_PARTIAL) SSDK_ATTR_G(64, EPI_SILU) SSDK_ATTR_G(64, EPI_PUBLISH)
@@ -1252,7 +1278,7 @@ int ssdk_bind_weight(ssdk_handle h, int which, int kind, int layer, const void* 
     if (rows != er || cols != ec)
       return fail("bind_weight kind %d layer %d: shape [%lld,%lld], expected [%lld,%lld]", kind, layer, (long long)rows,
                   (long long)cols, (long long)er, (long long)ec);
-    w.ptr = (const bf16*)dev_ptr; w.rows = rows; w.cols = cols; w.has_tm = false;
+    w.ptr = (const bf16*)dev_ptr; w.scale = nullptr; w.rows = rows; w.cols = cols; w.has_tm = false;
     return 0;
   };
   auto vec = [&](const bf16** dst, int64_t n) -> int {
@@ -1282,6 +1308,32 @@ int ssdk_bind_weight(ssdk_handle h, int which, int kind, int layer, const void* 
       return 0;
     default: return fail("bind_weight: unknown kind %d", kind);
   }
+}
+
+int ssdk_bind_weight_fp8(ssdk_handle h, int which, int kind, int layer, const void* w_e4m3, const float* row_scale,
+                         int64_t rows, int64_t cols) {
+  if (!h || which < 0 || which > 1 || !h->model[which].present) return fail("bind_weight_fp8: bad handle/model");
+  if (which != SSDK_TARGET) return fail("bind_weight_fp8: FP8 weights are supported for the target model only");
+  if (!w_e4m3 || !row_scale) return fail("bind_weight_fp8: null pointer");
+  Model& m = h->model[which];
+  if (layer < 0 || layer >= m.cfg.layers) return fail("bind_weight_fp8: layer %d out of range", layer);
+  LayerW& lw = m.layers[layer];
+  WeightMat* w = nullptr;
+  int64_t er = 0, ec = 0;
+  switch (kind) {
+    case SSDK_W_QKV: w = &lw.qkv; er = m.qkv_dim; ec = m.d; break;
+    case SSDK_W_O: w = &lw.o; er = m.d; ec = (int64_t)m.H * m.hd; break;
+    case SSDK_W_GATE_UP: w = &lw.gate_up; er = 2 * (int64_t)m.ffn; ec = m.d; break;
+    case SSDK_W_DOWN: w = &lw.down; er = m.d; ec = m.ffn; break;
+    default: return fail("bind_weight_fp8: kind %d has no FP8 form (qkv, o, gate_up and down only)", kind);
+  }
+  if (rows != er || cols != ec)
+    return fail("bind_weight_fp8 kind %d layer %d: shape [%lld,%lld], expected [%lld,%lld]", kind, layer, (long long)rows,
+                (long long)cols, (long long)er, (long long)ec);
+  if (cols % kBlockK8) return fail("bind_weight_fp8 kind %d: K=%lld is not a multiple of %d", kind, (long long)cols, kBlockK8);
+  if (((uintptr_t)w_e4m3 & 15) != 0) return fail("bind_weight_fp8: weight pointer not 16-byte aligned");
+  w->ptr = (const bf16*)w_e4m3; w->scale = row_scale; w->rows = rows; w->cols = cols; w->has_tm = false;
+  return 0;
 }
 
 int ssdk_bind_kv_cache(ssdk_handle h, int which, void* kv_base, int64_t num_blocks) {
@@ -1658,6 +1710,64 @@ int ssdk_gemm_gate_up_silu(const void* x, const void* w_gate_up, void* hout, int
   p.out = hout; p.M = M; p.N = ffn; p.ldo = ffn; p.num_kb = K / kBlockK; p.kb_per_split = p.num_kb;
   p.tile_rows = 64; p.hi_row_offset = ffn;
   return launch_gemm(L, un, EPI_SILU, tmW, tmX, p, (ffn + 63) / 64, 1);
+}
+
+int ssdk_gemm_small_m_fp8(const void* x, const void* w8, const float* scale, void* y, float* partials, int M, int N, int K,
+                          int ldy, int split_k, void* stream) {
+  if (M < 1 || M > kMaxTokens) return fail("gemm_small_m_fp8: M=%d out of [1,%d]", M, kMaxTokens);
+  if (K % kBlockK8) return fail("gemm_small_m_fp8: K=%d is not a multiple of %d", K, kBlockK8);
+  if (!scale) return fail("gemm_small_m_fp8: null scale");
+  Launcher L;
+  L.st = (cudaStream_t)stream;
+  CUtensorMap tmW, tmX;
+  CKI(make_tmap_e4m3(&tmW, w8, N, K));
+  const int un = umma_n_for(M);
+  CKI(make_tmap(&tmX, x, M, K, un));
+  const int tiles = (N + kTileRows - 1) / kTileRows;
+  const int num_kb = K / kBlockK8;
+  int S = split_k > 0 ? std::min(split_k, num_kb) : auto_splits(tiles, num_kb, un <= 64 ? 2 : 1);
+  if (S > 1 && !partials) return fail("gemm_small_m_fp8: split_k=%d needs a partials buffer", S);
+  GemmParams p;
+  p.M = M; p.N = N; p.ldo = ldy; p.num_kb = num_kb; p.tile_rows = kTileRows; p.hi_row_offset = 64;
+  p.kb_per_split = (num_kb + S - 1) / S;
+  S = (num_kb + p.kb_per_split - 1) / p.kb_per_split;
+  if (S == 1) {
+    p.out = y;
+    return launch_gemm(L, un, EPI_BF16, tmW, tmX, p, tiles, 1, scale);
+  }
+  p.out = partials;
+  CKI(launch_gemm(L, un, EPI_PARTIAL, tmW, tmX, p, tiles, S, scale));
+  const int n = M * N;
+  return L.go(splitk_reduce_kernel, dim3((n + 255) / 256), dim3(256), 0, (const float*)partials, (bf16*)y, S, M, N, ldy);
+}
+
+int ssdk_gemm_gate_up_silu_fp8(const void* x, const void* w8_gate_up, const float* scale, void* hout, float* partials,
+                               unsigned* counters, int M, int ffn, int K, int split_k, void* stream) {
+  if (M < 1 || M > kMaxTokens) return fail("gemm_gate_up_silu_fp8: M=%d out of range", M);
+  if (K % kBlockK8 || ffn % 8) return fail("gemm_gate_up_silu_fp8: K %% 128 or ffn %% 8 violated");
+  if (!scale) return fail("gemm_gate_up_silu_fp8: null scale");
+  Launcher L;
+  L.st = (cudaStream_t)stream;
+  CUtensorMap tmW, tmX;
+  CKI(make_tmap_e4m3(&tmW, w8_gate_up, 2 * (int64_t)ffn, K));
+  const int un = umma_n_for(M);
+  CKI(make_tmap(&tmX, x, M, K, un));
+  const int tiles = (ffn + 63) / 64;
+  GemmParams p;
+  memset(&p, 0, sizeof(p));
+  p.out = hout; p.M = M; p.N = ffn; p.ldo = ffn; p.num_kb = K / kBlockK8;
+  p.tile_rows = 64; p.hi_row_offset = ffn;
+  const int S = std::max(1, std::min(split_k, p.num_kb));
+  p.kb_per_split = (p.num_kb + S - 1) / S;
+  const int splits = (p.num_kb + p.kb_per_split - 1) / p.kb_per_split;
+  if (splits > 1) {
+    // in-kernel split-K (the engine's path for narrow tensor-parallel shards): fp32 [S, M, 2 ffn] partials and one
+    // zeroed ticket counter per 64-column tile
+    if (!partials || !counters) return fail("gemm_gate_up_silu_fp8: split_k=%d needs partials and counters", splits);
+    if (un > 64 || tiles > 512) return fail("gemm_gate_up_silu_fp8: split-K is planned for <= 64 tokens, <= 512 tiles");
+    p.sk_partials = partials; p.sk_counters = counters; p.sk_width = 2 * ffn;
+  }
+  return launch_gemm(L, un, EPI_SILU, tmW, tmX, p, tiles, splits, scale);
 }
 
 int ssdk_rmsnorm(const void* x, const void* residual_in, const void* w, float eps, void* y, void* residual_out, int M,

@@ -110,13 +110,22 @@ SSDK_DEVINL bool splitk_ticket_reduce(uint32_t* r, const GemmParams& p, int col,
 }
 
 
-template <int UMMA_N>
+// FP8 (e4m3) weights: a k-block is one 128-byte swizzle row of weight BYTES = 128 k, i.e. two bf16 k-blocks of X
+constexpr int kBlockK8 = 128;
+
+template <int UMMA_N, bool FP8 = false>
 struct GemmCfg {
-  static constexpr int kABytes = kTileRows * kBlockK * 2;  // 16384
-  static constexpr int kBBytes = UMMA_N * kBlockK * 2;     // 2048 / 4096 / 8192 / 16384 / 32768
+  static constexpr int kBlockKW = FP8 ? kBlockK8 : kBlockK;  // k per pipeline stage
+  static constexpr int kABytes = kTileRows * 128;          // 16384: 128 weight rows x one 128 B swizzle row
+  static constexpr int kBBytes = UMMA_N * kBlockKW * 2;    // bf16 X: one (bf16) or two (fp8) [UMMA_N x 64 k] boxes
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kStages = (UMMA_N == 16) ? 6 : (UMMA_N == 32 ? 5 : 4);
-  static constexpr int kSmemBytes = kStages * kStageBytes + 1024;  // + alignment slack
+  // FP8: each consumer warpgroup widens its 64 x 128 fp8 half-tile into a bf16 copy (two 64 x 64 swizzled sub-tiles)
+  // behind the stages, 2 x 16 KB.  Stage counts keep two CTAs per SM at UMMA_N <= 64 (3 / 3 / 2 stages = 48 / 48 / 32
+  // KB of weight bytes in flight per CTA, as many weights as 6 / 6 / 4 bf16 stages).
+  static constexpr int kConvBytes = FP8 ? kTileRows * kBlockK8 * 2 : 0;
+  static constexpr int kStages = FP8 ? (UMMA_N <= 32 ? 3 : (UMMA_N == 64 ? 2 : (UMMA_N == 128 ? 4 : 2)))
+                                     : ((UMMA_N == 16) ? 6 : (UMMA_N == 32 ? 5 : 4));
+  static constexpr int kSmemBytes = kStages * kStageBytes + kConvBytes + 1024;  // + alignment slack
   // UMMA_N <= 64 (decode / verify: weight streaming, two CTAs per SM keep ~190 KB of loads in flight); 128 / 256 (prefill
   // chunks and large batches: 128-192 KB of stages, one CTA per SM, the weights are read once per 128 / 256 tokens)
   static constexpr int kCtasPerSm = UMMA_N <= 64 ? 2 : 1;
@@ -125,13 +134,40 @@ struct GemmCfg {
   // epilogue shared memory, carved from the drained pipeline: accumulator stage [128][kEpiCols + 1] fp32, then the
   // SiLU exchange of the same size
   static constexpr int kEpiBytes = kTileRows * (kEpiCols + 1) * 4;
-  static_assert(2 * kEpiBytes <= kStages * kStageBytes, "epilogue staging must fit in the pipeline stages");
+  static_assert(2 * kEpiBytes <= kStages * kStageBytes + kConvBytes, "epilogue staging must fit in the pipeline stages");
+  static_assert(kSmemBytes * kCtasPerSm <= 227 * 1024 - 2048, "shared memory over the SM's capacity");
 };
 
-template <int UMMA_N, int EPI>
-__global__ void __launch_bounds__(kGemmThreads, GemmCfg<UMMA_N>::kCtasPerSm)
-gemm_ws_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmX, GemmParams p) {
-  using Cfg = GemmCfg<UMMA_N>;
+// 16 e4m3 codes -> 16 bf16, exactly: e4m3 -> f16 is exact (every e4m3 subnormal is an f16 normal) and f16 -> f32 ->
+// bf16 is exact for values of at most 4 significant bits and |x| <= 448, so no bf16 subnormal is ever produced
+SSDK_DEVINL void e4m3x16_to_bf16(const uint4& v, uint4& lo, uint4& hi) {
+  const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+  uint32_t o[8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const uint16_t pair = (uint16_t)(w[i >> 1] >> (16 * (i & 1)));
+    uint32_t h2;
+    asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(h2) : "h"(pair));
+    const float f0 = __half2float(__ushort_as_half((unsigned short)(h2 & 0xFFFFu)));
+    const float f1 = __half2float(__ushort_as_half((unsigned short)(h2 >> 16)));
+    uint32_t b2;
+    asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(b2) : "f"(f1), "f"(f0));
+    o[i] = b2;
+  }
+  lo = make_uint4(o[0], o[1], o[2], o[3]);
+  hi = make_uint4(o[4], o[5], o[6], o[7]);
+}
+
+// FP8 = false: bf16 weights, w_scale unused.  FP8 = true (W8A16, K a multiple of 128): tmW is a byte map of the e4m3
+// weights ([N, K] row-major, box 128 B x 64 rows, 128B swizzle), w_scale the fp32 per-row scales;
+// y[m, n] = s[n] * sum_k bf16(W8[n, k]) * x[m, k], the scale applied to the fp32 accumulator before every epilogue
+// (split-K partials are stored scaled).  FP8 is a template parameter of this one kernel (not a wrapper around a shared
+// device function) because that keeps the bf16 instances' SASS byte-identical to the kernel without FP8 support.
+template <int UMMA_N, int EPI, bool FP8>
+__global__ void __launch_bounds__(kGemmThreads, GemmCfg<UMMA_N, FP8>::kCtasPerSm)
+gemm_ws_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmX, GemmParams p,
+               const float* __restrict__ w_scale) {
+  using Cfg = GemmCfg<UMMA_N, FP8>;
   constexpr int kStages = Cfg::kStages;
   constexpr int CW = Cfg::kEpiCols;
 
@@ -175,7 +211,7 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ 
       for (int i = 0; i < pre; ++i) {
         uint8_t* a_s = smem + i * Cfg::kStageBytes;
         mbar_arrive_expect_tx(&full_bar[i], Cfg::kStageBytes);
-        const int k = (kb0 + i) * kBlockK;
+        const int k = (kb0 + i) * Cfg::kBlockKW;
         tma_load_2d(a_s, &tmW, &full_bar[i], k, row_lo, kEvictFirst);
         tma_load_2d(a_s + Cfg::kABytes / 2, &tmW, &full_bar[i], k, row_hi, kEvictFirst);
       }
@@ -183,7 +219,9 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ 
       trace_mark(TR_GEMM);
       for (int i = 0; i < pre; ++i) {
         uint8_t* b_s = smem + i * Cfg::kStageBytes + Cfg::kABytes;
-        tma_load_2d(b_s, &tmX, &full_bar[i], (kb0 + i) * kBlockK, 0, kEvictLast);
+        tma_load_2d(b_s, &tmX, &full_bar[i], (kb0 + i) * Cfg::kBlockKW, 0, kEvictLast);
+        if constexpr (FP8)
+          tma_load_2d(b_s + Cfg::kBBytes / 2, &tmX, &full_bar[i], (kb0 + i) * Cfg::kBlockKW + kBlockK, 0, kEvictLast);
       }
       for (int i = pre; i < nkb; ++i) {
         const int s = i % kStages;
@@ -191,10 +229,11 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ 
         mbar_wait(&empty_bar[s], ph ^ 1u);
         uint8_t* a_s = smem + s * Cfg::kStageBytes;
         mbar_arrive_expect_tx(&full_bar[s], Cfg::kStageBytes);
-        const int k = (kb0 + i) * kBlockK;
+        const int k = (kb0 + i) * Cfg::kBlockKW;
         tma_load_2d(a_s, &tmW, &full_bar[s], k, row_lo, kEvictFirst);
         tma_load_2d(a_s + Cfg::kABytes / 2, &tmW, &full_bar[s], k, row_hi, kEvictFirst);
         tma_load_2d(a_s + Cfg::kABytes, &tmX, &full_bar[s], k, 0, kEvictLast);
+        if constexpr (FP8) tma_load_2d(a_s + Cfg::kABytes + Cfg::kBBytes / 2, &tmX, &full_bar[s], k + kBlockK, 0, kEvictLast);
       }
     }
   } else {
@@ -210,6 +249,44 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ 
       const uint32_t ph = (uint32_t)(i / kStages) & 1u;
       mbar_wait(&full_bar[s], ph);
       uint8_t* a_s = smem + s * Cfg::kStageBytes;
+      if constexpr (FP8) {
+        // widen this warpgroup's 64 x 128 e4m3 half-tile into two 64 x 64 bf16 sub-tiles in the TMA's 128B-swizzled
+        // layout (16-byte chunk c of row r sits at chunk c ^ (r & 7)), then run the bf16 wgmma on them
+        const uint8_t* w8 = a_s + wg * (Cfg::kABytes / 2);
+        uint8_t* cv = smem + kStages * Cfg::kStageBytes + wg * (Cfg::kConvBytes / 2);
+        // every warp of the group is past the previous k-block's wgmma reads of `cv`
+        asm volatile("bar.sync %0, 128;" ::"r"(3 + wg) : "memory");
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          const int idx = (threadIdx.x & 127) + 128 * q;
+          const int r = idx >> 3, c = idx & 7;  // half-tile row, 16-byte chunk = k 16c .. 16c + 15
+          const uint4 v = *reinterpret_cast<const uint4*>(w8 + r * 128 + ((c ^ (r & 7)) << 4));
+          uint4 lo, hi;
+          e4m3x16_to_bf16(v, lo, hi);
+          uint8_t* dst = cv + (c >> 2) * (Cfg::kConvBytes / 4) + r * 128;  // sub-tile of k 0..63 / 64..127
+          const int c0 = 2 * (c & 3);
+          *reinterpret_cast<uint4*>(dst + ((c0 ^ (r & 7)) << 4)) = lo;
+          *reinterpret_cast<uint4*>(dst + (((c0 + 1) ^ (r & 7)) << 4)) = hi;
+        }
+        fence_proxy_async_smem();  // generic-proxy stores -> wgmma (async proxy) reads
+        asm volatile("bar.sync %0, 128;" ::"r"(3 + wg) : "memory");
+        const uint64_t bdesc = make_wgmma_desc_k128(a_s + Cfg::kABytes);
+        wgmma_fence();
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const uint64_t adesc = make_wgmma_desc_k128(cv + h * (Cfg::kConvBytes / 4));
+#pragma unroll
+          for (int k = 0; k < kBlockK / 16; ++k)
+#pragma unroll
+            for (int c = 0; c < Cfg::kPasses; ++c)
+              wgmma_bf16_ss<CW>(acc[c], adesc + (uint64_t)(2 * k),
+                                bdesc + (uint64_t)(h * (UMMA_N * 128 / 16) + 2 * k + c * (CW * 128 / 16)), 1u);
+        }
+        wgmma_commit();
+        wgmma_wait_all();
+        if (lane == 0) mbar_arrive(&empty_bar[s]);
+        continue;
+      }
       const uint64_t adesc = make_wgmma_desc_k128(a_s + wg * (Cfg::kABytes / 2));
       const uint64_t bdesc = make_wgmma_desc_k128(a_s + Cfg::kABytes);
       wgmma_fence();
@@ -253,6 +330,14 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ 
     uint32_t r[CW];
 #pragma unroll
     for (int m = 0; m < CW; ++m) r[m] = __float_as_uint(stage[row * LD + m]);
+    if constexpr (FP8) {
+      // weight row of this thread: gate / up row of output column row_lo + (row & 63) (SiLU), else row_lo + row
+      const int out_col = row_lo + (EPI == EPI_SILU ? (row & 63) : row);
+      const int wrow = (EPI == EPI_SILU && row >= 64) ? p.hi_row_offset + out_col : out_col;
+      const float sc = out_col < p.N ? __ldg(w_scale + wrow) : 0.f;
+#pragma unroll
+      for (int m = 0; m < CW; ++m) r[m] = __float_as_uint(__uint_as_float(r[m]) * sc);
+    }
 
     if (EPI == EPI_BF16) {
       const int n = row_lo + row;

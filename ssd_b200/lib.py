@@ -49,6 +49,7 @@ SIGNATURES: dict[str, tuple] = {
     "ssdk_create": (C.c_int, [C.POINTER(ModelCfg), C.POINTER(ModelCfg), C.POINTER(RuntimeCfg), C.POINTER(VP)]),
     "ssdk_destroy": (C.c_int, [VP]),
     "ssdk_bind_weight": (C.c_int, [VP, C.c_int, C.c_int, C.c_int, VP, C.c_int64, C.c_int64]),
+    "ssdk_bind_weight_fp8": (C.c_int, [VP, C.c_int, C.c_int, C.c_int, VP, VP, C.c_int64, C.c_int64]),
     "ssdk_bind_kv_cache": (C.c_int, [VP, C.c_int, VP, C.c_int64]),
     "ssdk_workspace_bytes": (C.c_int64, [VP]),
     "ssdk_bind_workspace": (C.c_int, [VP, VP, C.c_int64]),
@@ -74,6 +75,8 @@ SIGNATURES: dict[str, tuple] = {
     "ssdk_launch_count": (C.c_int64, [VP]),
     "ssdk_gemm_small_m": (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, VP]),
     "ssdk_gemm_gate_up_silu": (C.c_int, [VP, VP, VP, C.c_int, C.c_int, C.c_int, VP]),
+    "ssdk_gemm_small_m_fp8": (C.c_int, [VP, VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, VP]),
+    "ssdk_gemm_gate_up_silu_fp8": (C.c_int, [VP, VP, VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, VP]),
     "ssdk_rmsnorm": (C.c_int, [VP, VP, VP, C.c_float, VP, VP, C.c_int, C.c_int, VP]),
     "ssdk_rope_store_kv": (C.c_int, [VP, VP, VP, VP, VP, VP, C.c_float, VP, VP, VP, C.c_int, C.c_int, C.c_int,
                                      C.c_int, VP]),

@@ -12,6 +12,7 @@ import os
 import torch
 
 from . import lib as L
+from .quant import FP8_LINEARS, quantize_layers_
 from .runner import ModelSpec, PairRunner
 
 
@@ -23,16 +24,36 @@ def spec_from_config(hf) -> ModelSpec:
                      max_pos=hf.max_position_embeddings)
 
 
-def load_safetensors_weights(path: str, spec: ModelSpec, device, tp_size: int = 1, tp_rank: int = 0) -> dict:
+# decoder linears: checkpoint leaf -> (packed matrix, sub-matrix index); column-parallel ones pack q|k|v and gate|up
+_LINEAR_LEAVES = {
+    "self_attn.q_proj": ("qkv", 0), "self_attn.k_proj": ("qkv", 1), "self_attn.v_proj": ("qkv", 2),
+    "self_attn.o_proj": ("o", 0), "mlp.gate_proj": ("gate_up", 0), "mlp.up_proj": ("gate_up", 1),
+    "mlp.down_proj": ("down", 0),
+}
+
+
+def load_safetensors_weights(path: str, spec: ModelSpec, device, tp_size: int = 1, tp_rank: int = 0,
+                             allow_fp8: bool = True) -> dict:
+    """Packed per-rank weights.  bf16 / fp16 / fp32 tensors are loaded as bf16.  A float8_e4m3fn decoder linear
+    `<proj>.weight` stays e4m3 and pairs with `<proj>.weight_scale` (fp32 or bf16, shape [N, 1], [N], [1] or []); the
+    packed matrix then gets fp32 per-row scales lw[name + "_scale"] (a per-tensor scale is broadcast to its rows, so
+    q|k|v and gate|up with different per-tensor scales become one per-row vector).  `input_scale` / `input_scale_ub`
+    are activation scales of W8A8 kernels and are ignored (listed in w["ignored"]).  Block-wise scales
+    (`weight_scale_inv`) raise NotImplementedError, and so does any FP8 tensor when allow_fp8 is False (the draft)."""
     from safetensors import safe_open
 
     H, KV, hd = spec.heads // tp_size, spec.kv_heads // tp_size, spec.head_dim
     ffn, Vs, d = spec.ffn // tp_size, spec.vocab // tp_size, spec.hidden
-    bf = torch.bfloat16
+    bf, f8 = torch.bfloat16, torch.float8_e4m3fn
     w = {"layers": [dict() for _ in range(spec.layers)]}
-    for lw in w["layers"]:
-        lw["qkv"] = torch.empty((H + 2 * KV) * hd, d, dtype=bf, device=device)
-        lw["gate_up"] = torch.empty(2 * ffn, d, dtype=bf, device=device)
+    ignored: list[str] = []
+    # per packed matrix: (rows of each sub-matrix in the checkpoint, rows of each on this rank, shape on this rank,
+    # column-parallel?)
+    full_rows = {"qkv": [spec.heads * hd, spec.kv_heads * hd, spec.kv_heads * hd], "gate_up": [spec.ffn, spec.ffn],
+                 "o": [d], "down": [d]}
+    rank_rows = {"qkv": [H * hd, KV * hd, KV * hd], "gate_up": [ffn, ffn], "o": [d], "down": [d]}
+    shape = {"qkv": ((H + 2 * KV) * hd, d), "gate_up": (2 * ffn, d), "o": (d, H * hd), "down": (d, ffn)}
+    scales_seen: dict[tuple[int, str, int], bool] = {}
 
     def rows(t, n):  # column-parallel: shard output rows
         return t[tp_rank * n:(tp_rank + 1) * n]
@@ -40,10 +61,66 @@ def load_safetensors_weights(path: str, spec: ModelSpec, device, tp_size: int = 
     def cols(t, n):  # row-parallel: shard input columns
         return t[:, tp_rank * n:(tp_rank + 1) * n]
 
+    def packed(lw, name, dtype):
+        if name not in lw:
+            lw[name] = torch.empty(*shape[name], dtype=dtype, device=device)
+            if dtype == f8:
+                lw[name + "_scale"] = torch.empty(shape[name][0], dtype=torch.float32, device=device)
+        elif lw[name].dtype != dtype:
+            raise ValueError(f"{path}: the parts of packed {name} mix FP8 and non-FP8 weights")
+        return lw[name]
+
+    def put_linear(lw, name, part, t):
+        dst = packed(lw, name, f8 if t.dtype == f8 else bf)
+        if name in ("o", "down"):
+            dst.copy_(cols(t if t.dtype == f8 else t.to(bf), shape[name][1]).to(device))
+            return
+        r0 = sum(rank_rows[name][:part])
+        n = rank_rows[name][part]
+        dst[r0:r0 + n] = rows(t if t.dtype == f8 else t.to(bf), n).to(device)
+
+    def put_scale(lw, layer, name, part, t):
+        n_full = full_rows[name][part]
+        t = t.float().reshape(-1)
+        if t.numel() == 1:
+            t = t.expand(n_full)
+        elif t.numel() != n_full:
+            raise ValueError(f"{path}: layer {layer} {name} weight_scale has {t.numel()} elements; expected 1 or "
+                             f"{n_full} (per-tensor or per-channel)")
+        sc = packed(lw, name, f8)
+        r0, n = sum(rank_rows[name][:part]), rank_rows[name][part]
+        # column-parallel: the scales follow their rows; row-parallel (o, down): every rank keeps all output-row
+        # scales, since a row scale factors out of each rank's partial sum
+        sc_rank = rows(t, n) if name in ("qkv", "gate_up") else t
+        lw[name + "_scale"][r0:r0 + n] = sc_rank.to(device)
+        scales_seen[(layer, name, part)] = True
+
     for file in sorted(glob.glob(os.path.join(path, "*.safetensors"))):
         with safe_open(file, "pt", "cpu") as f:
             for name in f.keys():
-                t = f.get_tensor(name).to(bf)
+                if name.endswith(".weight_scale_inv"):
+                    raise NotImplementedError(f"{path}: {name}: block-wise FP8 scales are not supported (per-channel or "
+                                              "per-tensor scales only)")
+                if name.endswith(".input_scale") or name.endswith(".input_scale_ub"):
+                    ignored.append(name)  # activation scales: the FP8 path is weight-only
+                    continue
+                t = f.get_tensor(name)
+                if t.dtype == f8 and not allow_fp8:
+                    raise NotImplementedError(f"{path}: {name} is FP8; FP8 weights are supported for the target model "
+                                              "only (the draft runs in bf16)")
+                parts = name.split(".")
+                if name.startswith("model.layers.") and ".".join(parts[3:-1]) in _LINEAR_LEAVES and \
+                        parts[-1] in ("weight", "weight_scale"):
+                    layer = int(parts[2])
+                    lname, part = _LINEAR_LEAVES[".".join(parts[3:-1])]
+                    if parts[-1] == "weight_scale":
+                        put_scale(w["layers"][layer], layer, lname, part, t)
+                    else:
+                        put_linear(w["layers"][layer], lname, part, t)
+                    continue
+                if t.dtype == f8:
+                    raise NotImplementedError(f"{path}: {name} is FP8; only the decoder linears may be FP8")
+                t = t.to(bf)
                 if name == "model.embed_tokens.weight":
                     w["embed"] = rows(t, Vs).to(device).contiguous()
                 elif name == "lm_head.weight":
@@ -51,23 +128,8 @@ def load_safetensors_weights(path: str, spec: ModelSpec, device, tp_size: int = 
                 elif name == "model.norm.weight":
                     w["final_norm"] = t.to(device)
                 elif name.startswith("model.layers."):
-                    parts = name.split(".")
                     lw, leaf = w["layers"][int(parts[2])], ".".join(parts[3:])
-                    if leaf == "self_attn.q_proj.weight":
-                        lw["qkv"][:H * hd] = rows(t, H * hd).to(device)
-                    elif leaf == "self_attn.k_proj.weight":
-                        lw["qkv"][H * hd:(H + KV) * hd] = rows(t, KV * hd).to(device)
-                    elif leaf == "self_attn.v_proj.weight":
-                        lw["qkv"][(H + KV) * hd:] = rows(t, KV * hd).to(device)
-                    elif leaf == "self_attn.o_proj.weight":
-                        lw["o"] = cols(t, H * hd).to(device).contiguous()
-                    elif leaf == "mlp.gate_proj.weight":
-                        lw["gate_up"][:ffn] = rows(t, ffn).to(device)
-                    elif leaf == "mlp.up_proj.weight":
-                        lw["gate_up"][ffn:] = rows(t, ffn).to(device)
-                    elif leaf == "mlp.down_proj.weight":
-                        lw["down"] = cols(t, ffn).to(device).contiguous()
-                    elif leaf == "input_layernorm.weight":
+                    if leaf == "input_layernorm.weight":
                         lw["input_norm"] = t.to(device)
                     elif leaf == "post_attention_layernorm.weight":
                         lw["post_norm"] = t.to(device)
@@ -75,9 +137,21 @@ def load_safetensors_weights(path: str, spec: ModelSpec, device, tp_size: int = 
                         lw["q_norm"] = t.to(device)
                     elif leaf == "self_attn.k_norm.weight":
                         lw["k_norm"] = t.to(device)
+    for layer, lw in enumerate(w["layers"]):
+        for lname, sub in full_rows.items():
+            if lname in lw and lw[lname].dtype == f8:
+                missing = [p for p in range(len(sub)) if (layer, lname, p) not in scales_seen]
+                if missing:
+                    raise ValueError(f"{path}: layer {layer} {lname}: FP8 weight without weight_scale")
     if "lm_head" not in w:  # tie_word_embeddings (models/llama3.py:321-322)
         w["lm_head"] = w["embed"]
+    if ignored:
+        w["ignored"] = ignored
     return w
+
+
+def is_fp8(w: dict) -> bool:
+    return any(lw[n].dtype == torch.float8_e4m3fn for lw in w["layers"] for n in FP8_LINEARS)
 
 
 def shard_packed_weights(w: dict, spec: ModelSpec, tp_size: int, tp_rank: int) -> dict:
@@ -90,14 +164,27 @@ def shard_packed_weights(w: dict, spec: ModelSpec, tp_size: int, tp_rank: int) -
     out = {"embed": w["embed"][r * vs:(r + 1) * vs].contiguous(), "lm_head": w["lm_head"][r * vs:(r + 1) * vs].contiguous(),
            "final_norm": w["final_norm"], "layers": []}
     for lw in w["layers"]:
-        q, k, v = lw["qkv"].split([H * hd, KV * hd, KV * hd], dim=0)
-        gate, up = lw["gate_up"].chunk(2, dim=0)
+        def col_par(name, t):  # q|k|v and gate|up rows (and their FP8 row scales) sliced per sub-matrix
+            if name == "qkv":
+                q, k, v = t.split([H * hd, KV * hd, KV * hd], dim=0)
+                return torch.cat([q[r * h * hd:(r + 1) * h * hd], k[r * kv * hd:(r + 1) * kv * hd],
+                                  v[r * kv * hd:(r + 1) * kv * hd]]).contiguous()
+            gate, up = t.chunk(2, dim=0)
+            return torch.cat([gate[r * f:(r + 1) * f], up[r * f:(r + 1) * f]]).contiguous()
+
         o = {"input_norm": lw["input_norm"], "post_norm": lw["post_norm"],
-             "qkv": torch.cat([q[r * h * hd:(r + 1) * h * hd], k[r * kv * hd:(r + 1) * kv * hd],
-                               v[r * kv * hd:(r + 1) * kv * hd]]).contiguous(),
+             "qkv": col_par("qkv", lw["qkv"]),
              "o": lw["o"][:, r * h * hd:(r + 1) * h * hd].contiguous(),
-             "gate_up": torch.cat([gate[r * f:(r + 1) * f], up[r * f:(r + 1) * f]]).contiguous(),
+             "gate_up": col_par("gate_up", lw["gate_up"]),
              "down": lw["down"][:, r * f:(r + 1) * f].contiguous()}
+        # FP8 row scales: column-parallel ones follow their rows; row-parallel (o, down) ones are replicated, since a
+        # row scale factors out of each rank's partial sum
+        for name in ("qkv", "gate_up"):
+            if name + "_scale" in lw:
+                o[name + "_scale"] = col_par(name, lw[name + "_scale"])
+        for name in ("o", "down"):
+            if name + "_scale" in lw:
+                o[name + "_scale"] = lw[name + "_scale"]
         for k2 in ("q_norm", "k_norm"):
             if k2 in lw:
                 o[k2] = lw[k2]
@@ -105,15 +192,35 @@ def shard_packed_weights(w: dict, spec: ModelSpec, tp_size: int, tp_rank: int) -
     return out
 
 
-def load_weights(path: str, spec: ModelSpec, device, tp_size: int = 1, tp_rank: int = 0) -> dict:
+def tp_row_amax_max(amax: torch.Tensor) -> torch.Tensor:
+    import torch.distributed as dist
+    dist.all_reduce(amax, op=dist.ReduceOp.MAX)
+    return amax
+
+
+def load_weights(path: str, spec: ModelSpec, device, tp_size: int = 1, tp_rank: int = 0,
+                 quantization: str | None = None, is_target: bool = True) -> dict:
+    """Packed per-rank weights of a synthetic directory or a safetensors checkpoint.  quantization="fp8" (target
+    only) replaces the decoder linears by e4m3 + per-row scales (quant.py) after loading, one tensor at a time; FP8
+    checkpoint tensors are kept as they are either way.  With tp_size > 1 every rank must call this together: the row
+    scales of o / down come from the full rows (a MAX all-reduce over the ranks' column shards)."""
+    if quantization is not None and not is_target:
+        raise NotImplementedError("quantization applies to the target model only (the draft runs in bf16)")
     marker = os.path.join(path, "ssd_b200_synthetic.json")
     if os.path.exists(marker):
         from .synth import generate_weights
         with open(marker) as f:
-            return generate_weights(spec, json.load(f), device, tp_size, tp_rank)
-    if glob.glob(os.path.join(path, "*.safetensors")):
-        return load_safetensors_weights(path, spec, device, tp_size, tp_rank)
-    raise FileNotFoundError(f"{path}: neither *.safetensors nor ssd_b200_synthetic.json")
+            w = generate_weights(spec, json.load(f), device, tp_size, tp_rank)
+    elif glob.glob(os.path.join(path, "*.safetensors")):
+        w = load_safetensors_weights(path, spec, device, tp_size, tp_rank, allow_fp8=is_target)
+    else:
+        raise FileNotFoundError(f"{path}: neither *.safetensors nor ssd_b200_synthetic.json")
+    if quantization == "fp8":
+        quantize_layers_(w, tp_row_amax_max if tp_size > 1 else None)
+        # the freed bf16 matrices and fp32 temporaries go back to the device, so that kv_blocks_for sees them as free
+        if torch.device(device).type == "cuda":
+            torch.cuda.empty_cache()
+    return w
 
 
 class _DraftCfg:
@@ -142,8 +249,10 @@ def build_runner(config, tp_size: int = 1, tp_rank: int = 0, device=None, finali
     torch.cuda.set_device(device)
     tspec = spec_from_config(config.hf_config)
     dspec = spec_from_config(config.draft_hf_config) if config.speculate else None
-    wt = load_weights(config.model, tspec, device, tp_size, tp_rank)
-    wd = load_weights(config.draft, dspec, device) if (dspec is not None and tp_rank == 0) else None
+    wt = load_weights(config.model, tspec, device, tp_size, tp_rank, quantization=config.quantization)
+    if is_fp8(wt):  # an FP8 checkpoint found by its tensor dtypes
+        config.quantization = "fp8"
+    wd = load_weights(config.draft, dspec, device, is_target=False) if (dspec is not None and tp_rank == 0) else None
     if dspec is not None and tp_rank != 0:
         dspec = None  # the draft is a replica pinned to rank 0 (SURVEY §8e)
     nbt = kv_blocks_for(config, tspec, tp_size, 0.8 if dspec else 1.0)

@@ -71,6 +71,53 @@ def gate_up_silu(x: torch.Tensor, w_gate_up: torch.Tensor) -> torch.Tensor:
     return h
 
 
+def linear_fp8(x: torch.Tensor, w8: torch.Tensor, scale: torch.Tensor, split_k: int = 0) -> torch.Tensor:
+    """y = bf16(scale[n] * x @ bf16(w8)^T) for M = x.shape[0] <= 256 tokens (FP8 weight-only GEMM; the reference has no
+    FP8 path).  x [M, K] bf16, w8 [N, K] float8_e4m3fn, scale [N] fp32, K a multiple of 128.  split_k as in `linear`."""
+    _req(x, torch.bfloat16, "x")
+    _req(w8, torch.float8_e4m3fn, "w8")
+    _req(scale, torch.float32, "scale")
+    M, K = x.shape
+    N = w8.shape[0]
+    assert w8.shape[1] == K and scale.numel() == N
+    y = torch.empty(M, N, dtype=torch.bfloat16, device=x.device)
+    nkb = K // 128
+    if split_k == 1:
+        parts = None
+    else:
+        if split_k == 0:  # same bound as auto_splits() in csrc/engine.cu
+            tiles = (N + 127) // 128
+            sms = torch.cuda.get_device_properties(x.device).multi_processor_count
+            s_bound = max(1, min(max(1, nkb // 4), (2 * sms + tiles - 1) // tiles))
+        else:
+            s_bound = min(split_k, nkb)
+        parts = torch.empty(s_bound * M * N, dtype=torch.float32, device=x.device)
+    lib = _L.load()
+    _L.check(lib.ssdk_gemm_small_m_fp8(_ptr(x), _ptr(w8), _ptr(scale), _ptr(y), _ptr(parts), M, N, K, N, split_k,
+                                       _stream()), "ssdk_gemm_small_m_fp8")
+    return y
+
+
+def gate_up_silu_fp8(x: torch.Tensor, w8_gate_up: torch.Tensor, scale: torch.Tensor, split_k: int = 1) -> torch.Tensor:
+    """`gate_up_silu` with FP8 weights: w8_gate_up [2*ffn, K] float8_e4m3fn (gate rows then up rows), scale [2*ffn]
+    fp32.  split_k > 1 (M <= 64) runs the in-kernel split-K reduction the engine uses for narrow tensor-parallel shards."""
+    _req(x, torch.bfloat16, "x")
+    _req(w8_gate_up, torch.float8_e4m3fn, "w8_gate_up")
+    _req(scale, torch.float32, "scale")
+    M, K = x.shape
+    ffn = w8_gate_up.shape[0] // 2
+    assert scale.numel() == 2 * ffn
+    h = torch.empty(M, ffn, dtype=torch.bfloat16, device=x.device)
+    parts = counters = None
+    if split_k > 1:
+        parts = torch.empty(split_k * M * 2 * ffn, dtype=torch.float32, device=x.device)
+        counters = torch.zeros((ffn + 63) // 64, dtype=torch.int32, device=x.device)
+    lib = _L.load()
+    _L.check(lib.ssdk_gemm_gate_up_silu_fp8(_ptr(x), _ptr(w8_gate_up), _ptr(scale), _ptr(h), _ptr(parts), _ptr(counters),
+                                            M, ffn, K, split_k, _stream()), "ssdk_gemm_gate_up_silu_fp8")
+    return h
+
+
 def rms_norm(x: torch.Tensor, weight: torch.Tensor, eps: float, residual: torch.Tensor | None = None):
     """RMSDNorm.forward (layers/layernorm.py:90-98).  Returns y if residual is None else (y, new_residual)."""
     _req(x, torch.bfloat16, "x")

@@ -125,10 +125,19 @@ class PairRunner:
     # ------------------------------------------------------------------ weights
     def bind_weights(self, which: int, w: dict) -> None:
         """w: packed per-rank tensors on this device (bf16):
-        embed, lm_head, final_norm, layers[l] = {input_norm, qkv, o, post_norm, gate_up, down[, q_norm, k_norm]}."""
+        embed, lm_head, final_norm, layers[l] = {input_norm, qkv, o, post_norm, gate_up, down[, q_norm, k_norm]}.
+        A decoder linear of the target may instead be float8_e4m3fn with fp32 row scales in layers[l][name + "_scale"]
+        (quant.py); it is bound with ssdk_bind_weight_fp8."""
         lib, h = self.lib, self.h
 
-        def bind(kind, layer, t):
+        def bind(kind, layer, t, scale=None):
+            if t.dtype == torch.float8_e4m3fn:
+                if scale is None or scale.dtype != torch.float32 or not (t.is_cuda and scale.is_cuda) or \
+                        not (t.is_contiguous() and scale.is_contiguous()):
+                    raise ValueError("FP8 weights need contiguous CUDA tensors and fp32 row scales")
+                L.check(lib.ssdk_bind_weight_fp8(h, which, kind, layer, t.data_ptr(), scale.data_ptr(), t.shape[0],
+                                                 t.shape[1]), f"bind fp8 kind={kind} layer={layer}")
+                return
             if t.dtype != torch.bfloat16 or not t.is_cuda or not t.is_contiguous():
                 raise ValueError("weights must be contiguous bf16 CUDA tensors")
             rows, cols = (t.shape[0], t.shape[1]) if t.dim() == 2 else (t.shape[0], 1)
@@ -139,11 +148,11 @@ class PairRunner:
         bind(L.W_FINAL_NORM, 0, w["final_norm"])
         for l, lw in enumerate(w["layers"]):
             bind(L.W_INPUT_NORM, l, lw["input_norm"])
-            bind(L.W_QKV, l, lw["qkv"])
-            bind(L.W_O, l, lw["o"])
+            bind(L.W_QKV, l, lw["qkv"], lw.get("qkv_scale"))
+            bind(L.W_O, l, lw["o"], lw.get("o_scale"))
             bind(L.W_POST_NORM, l, lw["post_norm"])
-            bind(L.W_GATE_UP, l, lw["gate_up"])
-            bind(L.W_DOWN, l, lw["down"])
+            bind(L.W_GATE_UP, l, lw["gate_up"], lw.get("gate_up_scale"))
+            bind(L.W_DOWN, l, lw["down"], lw.get("down_scale"))
             if "q_norm" in lw:
                 bind(L.W_Q_NORM, l, lw["q_norm"])
                 bind(L.W_K_NORM, l, lw["k_norm"])
