@@ -78,7 +78,8 @@ typedef struct ssdk_runtime_cfg {
   int32_t use_graph;          /* 1 = capture the spec step into one CUDA graph */
   int32_t use_pdl;            /* 1 = programmatic dependent launch between kernels */
   int32_t jit_speculate;      /* verify(): ratio acceptance on every temp>0 row (utils/verify.py:59-62) */
-  int32_t reserved;
+  int32_t draft_fp8;          /* 0 = bf16 draft; 1 = the draft's decoder linears are FP8 (ssdk_bind_weight_fp8),
+                                 all of them: ssdk_finalize refuses a draft that is bf16 or only partly FP8 */
 } ssdk_runtime_cfg;
 
 /* ---- lifetime ------------------------------------------------------------- */
@@ -98,9 +99,10 @@ int ssdk_destroy(ssdk_handle h);
 int ssdk_bind_weight(ssdk_handle h, int which, int kind, int layer,
                      const void* dev_ptr, int64_t rows, int64_t cols);
 
-/* FP8 weight-only (W8A16) form of a target decoder linear.  The reference has
+/* FP8 weight-only (W8A16) form of a decoder linear.  The reference has
  * no FP8 path.  kind: SSDK_W_QKV, SSDK_W_O, SSDK_W_GATE_UP or SSDK_W_DOWN;
- * which: SSDK_TARGET only (the draft stays bf16).  Layout, no packing step:
+ * which: SSDK_TARGET, or SSDK_DRAFT when the runtime config sets draft_fp8 = 1
+ * (then every decoder linear of the draft must be FP8).  Layout, no packing step:
  *   w_e4m3    float8 e4m3fn [rows, cols] row-major, same shape and row order as
  *             the bf16 matrix of that kind (q|k|v and gate|up packed), 16-byte aligned;
  *   row_scale fp32 [rows]: row n of the matrix is row_scale[n] * W8[n, :].

@@ -54,6 +54,11 @@ class Config:
     # (W8A16, DESIGN.md §3); bf16 checkpoints are quantized on load.  This changes the outputs.  An FP8 checkpoint is
     # loaded as FP8 whatever this says, and the field then reads "fp8".
     quantization: str | None = None
+    # "fp8": the same for the draft's four decoder linears, independently of `quantization`.  At temperature 0 the engine
+    # still emits the target's greedy chain and at temperature > 0 it still samples the target's distribution: an FP8
+    # draft changes only the acceptance rate and the speed.  An FP8 draft checkpoint is loaded as FP8 whatever this says,
+    # and the field then reads "fp8".
+    draft_quantization: str | None = None
 
     @property
     def max_blocks(self) -> int:
@@ -71,6 +76,7 @@ class Config:
         if self.enforce_eager:
             self.use_cuda_graph = False
         self.quantization = parse_quantization(self.quantization)
+        self.draft_quantization = parse_quantization(self.draft_quantization)
         self.hf_config = load_hf_config(self.model)
         if checkpoint_quantization(self.hf_config) == "fp8":
             self.quantization = "fp8"
@@ -79,9 +85,8 @@ class Config:
             if not os.path.isdir(self.draft):
                 raise AssertionError(f"draft directory {self.draft!r} does not exist")
             self.draft_hf_config = load_hf_config(self.draft)
-            if getattr(self.draft_hf_config, "quantization_config", None):
-                raise NotImplementedError(f"{self.draft}: quantized draft checkpoints are not supported (the draft runs "
-                                          "in bf16)")
+            if checkpoint_quantization(self.draft_hf_config) == "fp8":  # any other quantization raises
+                self.draft_quantization = "fp8"
             self.max_model_len = min(self.max_model_len, self.draft_hf_config.max_position_embeddings)
         if self.max_num_batched_tokens < self.max_model_len:
             raise AssertionError("max_num_batched_tokens < max_model_len (config.py:94)")

@@ -43,6 +43,17 @@
 //   gate|up    : 8 (gate, up) row pairs = two slots (8 gate rows | the 8 matching up rows); warp w owns pair w.
 //   K >  2048  : R = 4 (K <= 4096) or 2 (K <= 8192) rows = one slot; the 8 warps split (row, K-segment) units and combine
 //                their partial sums in a fixed order through shared memory.
+//
+// FP8 (draft_stream_kernel<HD, GMAX, true>): the four decoder linears are e4m3 bytes with fp32 per-row scales (quant.py);
+// the lm_head stays bf16 and keeps the geometry above.  A lane reads 8 e4m3 bytes per 256-column step (one 8-byte shared
+// load, conflict-free) where the bf16 path reads 16 bytes, so it keeps the same 8 columns per lane, the same x slice in
+// registers (at most 64 floats) and the same per-lane and shuffle summation order.  A row then takes half the slot bytes, so
+// every job carries TWICE the rows of its bf16 form and each warp owns two rows (w and w + 8, or the second R-row group of a
+// split job): 16 rows per slot for K <= 2048, 16 gate|up pairs per two slots, 8 (K <= 4096) or 4 (K <= 8192) rows per slot
+// above.  Slots stay full, so the bytes in flight per SM are the bf16 ring's.  Each warp widens e4m3 -> f16 -> f32 on the
+// CUDA cores (exact), and the row scale multiplies the finished fp32 dot product (split rows: the segment sum) right
+// before the one bf16 rounding: y[n] = bf16(s[n] * sum_k W8[n, k] x[k]).  gate and up are scaled each by its own scale
+// before SiLU.
 #pragma once
 #include "common.cuh"
 #include "sampling.cuh"
@@ -92,6 +103,9 @@ struct DsParams {
   DsLayer layers[kDsMaxLayers];
   const int64_t* pend_tok;       // [1] (may be null): >= 0: the token at position ctx0 - 1, whose KV forward 0 writes as row 0
   __nv_bfloat16* vec_row0;       // row 0's vectors (ds_row0_vecs layout); read only when a token is pending
+  // FP8 instance only: fp32 per-row scales of layer l's qkv / o / gate_up / down (indexed by DS_QKV .. DS_DOWN); the
+  // DsLayer pointers of these four matrices then point at e4m3 bytes
+  const float* fp8_scale[kDsMaxLayers][4];
 };
 
 // vectors of row 0 of a two-row forward 0, carved from p.vec_row0 like the engine carves the row-1 vectors
@@ -196,6 +210,13 @@ __host__ SSDK_DEVINL bool ds_geometry(int K, int rows, bool pair, DsGeom* g) {
   g->nj = (rows + g->rpj - 1) / g->rpj;
   return true;
 }
+// an FP8 decoder linear: the bf16 job shape (segments, x layout) with twice the rows per job (see the top of the file)
+__host__ SSDK_DEVINL bool ds_geometry8(int K, int rows, bool pair, DsGeom* g) {
+  if (!ds_geometry(K, rows, pair, g)) return false;
+  g->rpj *= 2;
+  g->nj = (rows + g->rpj - 1) / g->rpj;
+  return true;
+}
 SSDK_DEVINL bool ds_has_head(const DsParams& p, int f) { return !(p.skip_last_head && f == p.n_fwd - 1); }
 SSDK_DEVINL const __nv_bfloat16* ds_weight(const DsParams& p, int l, int m) {
   const DsLayer& lw = p.layers[l < p.L ? l : 0];
@@ -232,6 +253,8 @@ SSDK_DEVINL void ds_cursor_next(const DsParams& p, const DsGeom* geom, DsCursor&
   c.s += (int)gridDim.x;
   if (c.s >= geom[c.m].nj) ds_cursor_settle(p, geom, c);
 }
+// FP8: the decoder linears are e4m3 (one byte per weight), the lm_head bf16
+template <bool FP8>
 SSDK_DEVINL void ds_producer(const DsParams& p, const DsGeom* geom, uint8_t* ring, uint64_t* full, uint64_t* empty) {
   DsCursor c;
   c.f = 0; c.l = 0; c.m = DS_QKV; c.s = (int)blockIdx.x; c.valid = p.n_fwd > 0;
@@ -242,13 +265,20 @@ SSDK_DEVINL void ds_producer(const DsParams& p, const DsGeom* geom, uint8_t* rin
     const DsGeom g = geom[c.m];
     const __nv_bfloat16* w = ds_weight(p, c.l, c.m);
     const int rows = min(g.rpj, g.rows - c.s * g.rpj);
-    const unsigned bytes = (unsigned)rows * (unsigned)g.K * 2u;
+    unsigned bytes = (unsigned)rows * (unsigned)g.K * 2u;
+    if constexpr (FP8) {
+      if (c.m != DS_HEAD) bytes >>= 1;
+    }
     const int parts = g.kind == DS_PAIR ? 2 : 1;
     for (int q = 0; q < parts; ++q) {
       const unsigned slot = n % S, round = n / S;
       mbar_wait(&empty[slot], (round & 1u) ^ 1u);  // a fresh barrier passes the first round at once
       mbar_arrive_expect_tx(&full[slot], bytes);
-      const __nv_bfloat16* src = w + ((size_t)(q ? g.rows : 0) + (size_t)c.s * g.rpj) * g.K;
+      const void* src = w + ((size_t)(q ? g.rows : 0) + (size_t)c.s * g.rpj) * g.K;
+      if constexpr (FP8) {
+        if (c.m != DS_HEAD)
+          src = reinterpret_cast<const uint8_t*>(w) + ((size_t)(q ? g.rows : 0) + (size_t)c.s * g.rpj) * g.K;
+      }
       bulk_load_g2s(ring + (size_t)slot * kDsSlotBytes, src, bytes, &full[slot]);
       ++n;
     }
@@ -312,6 +342,45 @@ SSDK_DEVINL float ds_dot_seg(const uint8_t* wseg, int steps, int lane, const flo
   return warp_sum((a0 + a1) + (a2 + a3));
 }
 
+// the two e4m3 codes in the low 16 bits of v (the lower byte is the first) -> two floats, exactly: e4m3 -> f16 is exact
+// (every e4m3 subnormal is an f16 normal), and so is f16 -> f32
+SSDK_DEVINL float2 ds_e4m3x2(uint32_t v) {
+#ifdef SSDK_HOST_EMU
+  auto one = [](uint32_t b) {
+    const int e = (int)((b >> 3) & 15u), m = (int)(b & 7u);
+    float x = (e == 15 && m == 7) ? NAN : (e ? std::ldexp(1.0f + (float)m / 8.0f, e - 7) : std::ldexp((float)m, -9));
+    return (b & 0x80u) ? -x : x;
+  };
+  return make_float2(one(v & 0xFFu), one((v >> 8) & 0xFFu));
+#else
+  uint32_t h2;
+  asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(h2) : "h"((unsigned short)(v & 0xFFFFu)));
+  return make_float2(__half2float(__ushort_as_half((unsigned short)(h2 & 0xFFFFu))),
+                     __half2float(__ushort_as_half((unsigned short)(h2 >> 16))));
+#endif
+}
+// ds_dot_seg for an e4m3 row segment: 8 bytes (the same 8 columns) per lane per step, the same summation order; the
+// caller applies the row scale
+SSDK_DEVINL float ds_dot_seg8(const uint8_t* wseg, int steps, int lane, const float (&xr)[kDsMaxSteps][8]) {
+  const uint2* wp = reinterpret_cast<const uint2*>(wseg) + lane;
+  float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
+#pragma unroll
+  for (int j = 0; j < kDsMaxSteps; ++j) {
+    if (j < steps) {
+      const uint2 w = wp[j * 32];
+      float2 f = ds_e4m3x2(w.x);
+      a0 = fmaf(f.x, xr[j][0], a0); a1 = fmaf(f.y, xr[j][1], a1);
+      f = ds_e4m3x2(w.x >> 16);
+      a2 = fmaf(f.x, xr[j][2], a2); a3 = fmaf(f.y, xr[j][3], a3);
+      f = ds_e4m3x2(w.y);
+      a0 = fmaf(f.x, xr[j][4], a0); a1 = fmaf(f.y, xr[j][5], a1);
+      f = ds_e4m3x2(w.y >> 16);
+      a2 = fmaf(f.x, xr[j][6], a2); a3 = fmaf(f.y, xr[j][7], a3);
+    }
+  }
+  return warp_sum((a0 + a1) + (a2 + a3));
+}
+
 // sampling state of the lm_head phase (lane 0 of every consumer warp follows its own rows)
 struct DsSample {
   bool greedy;
@@ -350,6 +419,26 @@ SSDK_DEVINL float ds_dot_seg0(const uint8_t* wseg, int steps, int lane, const fl
     f = ds_bf2(w.z);
     a0 = fmaf(f.x, v.x, a0); a1 = fmaf(f.y, v.y, a1);
     f = ds_bf2(w.w);
+    a2 = fmaf(f.x, v.z, a2); a3 = fmaf(f.y, v.w, a3);
+  }
+  return warp_sum((a0 + a1) + (a2 + a3));
+}
+// the same for an e4m3 row segment (ds_dot_seg8's arithmetic)
+SSDK_DEVINL float ds_dot_seg08(const uint8_t* wseg, int steps, int lane, const float* x0) {
+  const uint2* wp = reinterpret_cast<const uint2*>(wseg) + lane;
+  float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
+#pragma unroll 2
+  for (int j = 0; j < steps; ++j) {
+    const float4 u = *reinterpret_cast<const float4*>(x0 + j * 256 + lane * 8);
+    const float4 v = *reinterpret_cast<const float4*>(x0 + j * 256 + lane * 8 + 4);
+    const uint2 w = wp[j * 32];
+    float2 f = ds_e4m3x2(w.x);
+    a0 = fmaf(f.x, u.x, a0); a1 = fmaf(f.y, u.y, a1);
+    f = ds_e4m3x2(w.x >> 16);
+    a2 = fmaf(f.x, u.z, a2); a3 = fmaf(f.y, u.w, a3);
+    f = ds_e4m3x2(w.y);
+    a0 = fmaf(f.x, v.x, a0); a1 = fmaf(f.y, v.y, a1);
+    f = ds_e4m3x2(w.y >> 16);
     a2 = fmaf(f.x, v.z, a2); a3 = fmaf(f.y, v.w, a3);
   }
   return warp_sum((a0 + a1) + (a2 + a3));
@@ -474,20 +563,180 @@ SSDK_DEVINL void ds_consume_split(DsRing& ring, const DsGeom& g, float* xs, floa
     }
   }
 }
-// two: two rows (row 0 = r0)
-SSDK_DEVINL void ds_consume(DsRing& ring, const DsGeom& g, float* xs, float* res, __nv_bfloat16* y, bool two,
-                            const DsRow0& r0) {
-  if (g.kind == DS_PLAIN) {
-    if (two) ds_consume_plain<false, true>(ring, g, xs, y, nullptr, r0);
-    else ds_consume_plain<false>(ring, g, xs, y, nullptr);
-  } else {
-    if (two) ds_consume_split<true>(ring, g, xs, res, y, r0);
-    else ds_consume_split<false>(ring, g, xs, res, y, r0);
+
+// ---- FP8 (e4m3) forms of the three consume shapes: two rows per warp (see the top of the file), each output
+//      y = bf16(s * dot) with the row scale s requested before the slot is waited for ----
+// K <= 2048: 16 rows per slot, warp w owns rows w and w + 8
+template <bool TWO>
+SSDK_DEVINL void ds_consume_plain8(DsRing& ring, const DsGeom& g, float* xs, __nv_bfloat16* y, const DsRow0& r0,
+                                   const float* scale) {
+  if ((int)blockIdx.x >= g.nj) return;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int steps = g.K >> 8;
+  float xr[kDsMaxSteps][8];
+  ds_load_x(xs, steps, lane, xr);
+  const float* x0 = nullptr;
+  if constexpr (TWO) x0 = ds_row0_x(r0, xs, g.K);
+  for (int s = (int)blockIdx.x; s < g.nj; s += (int)gridDim.x) {
+    const int ra = s * 16 + warp, rb = ra + 8;
+    const float sa = ra < g.rows ? scale[ra] : 0.f, sb = rb < g.rows ? scale[rb] : 0.f;
+    const uint8_t* wa = ds_acquire(ring, 0) + (size_t)warp * g.K;
+    const uint8_t* wb = wa + (size_t)8 * g.K;
+    const float acc_a = ds_dot_seg8(wa, steps, lane, xr);
+    const float acc_b = ds_dot_seg8(wb, steps, lane, xr);
+    float acc0_a = 0.f, acc0_b = 0.f;
+    if constexpr (TWO) {
+      acc0_a = ds_dot_seg08(wa, steps, lane, x0);
+      acc0_b = ds_dot_seg08(wb, steps, lane, x0);
+    }
+    ds_release(ring, 0, lane);
+    ring.taken += 1u;
+    if (lane == 0) {
+      if (ra < g.rows) {
+        y[ra] = f2bf(acc_a * sa);
+        if constexpr (TWO) r0.y[ra] = f2bf(acc0_a * sa);
+      }
+      if (rb < g.rows) {
+        y[rb] = f2bf(acc_b * sb);
+        if constexpr (TWO) r0.y[rb] = f2bf(acc0_b * sb);
+      }
+    }
   }
 }
-SSDK_DEVINL void ds_consume_gu(DsRing& ring, const DsGeom& g, float* xs, __nv_bfloat16* act, bool two, const DsRow0& r0) {
-  if (two) ds_consume_pair<true>(ring, g, xs, act, r0);
-  else ds_consume_pair<false>(ring, g, xs, act, r0);
+// gate|up: 16 pairs per job (16 gate rows | the 16 matching up rows), warp w owns pairs w and w + 8; gate and up are
+// scaled each by its own row scale (scale[i] and scale[g.rows + i]) before SiLU
+template <bool TWO>
+SSDK_DEVINL void ds_consume_pair8(DsRing& ring, const DsGeom& g, float* xs, __nv_bfloat16* act, const DsRow0& r0,
+                                  const float* scale) {
+  if ((int)blockIdx.x >= g.nj) return;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int steps = g.K >> 8;
+  float xr[kDsMaxSteps][8];
+  ds_load_x(xs, steps, lane, xr);
+  const float* x0 = nullptr;
+  if constexpr (TWO) x0 = ds_row0_x(r0, xs, g.K);
+  for (int s = (int)blockIdx.x; s < g.nj; s += (int)gridDim.x) {
+    const int ia = s * 16 + warp, ib = ia + 8;
+    const float sga = ia < g.rows ? scale[ia] : 0.f, sua = ia < g.rows ? scale[g.rows + ia] : 0.f;
+    const float sgb = ib < g.rows ? scale[ib] : 0.f, sub = ib < g.rows ? scale[g.rows + ib] : 0.f;
+    float ga0 = 0.f, gb0 = 0.f, ua0 = 0.f, ub0 = 0.f;
+    const uint8_t* sg = ds_acquire(ring, 0) + (size_t)warp * g.K;
+    const float ga = ds_dot_seg8(sg, steps, lane, xr);
+    const float gb = ds_dot_seg8(sg + (size_t)8 * g.K, steps, lane, xr);
+    if constexpr (TWO) {
+      ga0 = ds_dot_seg08(sg, steps, lane, x0);
+      gb0 = ds_dot_seg08(sg + (size_t)8 * g.K, steps, lane, x0);
+    }
+    ds_release(ring, 0, lane);
+    const uint8_t* su = ds_acquire(ring, 1) + (size_t)warp * g.K;
+    const float ua = ds_dot_seg8(su, steps, lane, xr);
+    const float ub = ds_dot_seg8(su + (size_t)8 * g.K, steps, lane, xr);
+    if constexpr (TWO) {
+      ua0 = ds_dot_seg08(su, steps, lane, x0);
+      ub0 = ds_dot_seg08(su + (size_t)8 * g.K, steps, lane, x0);
+    }
+    ds_release(ring, 1, lane);
+    ring.taken += 2u;
+    if (lane == 0) {
+      if (ia < g.rows) {
+        act[ia] = f2bf(ds_silu_mul(ga * sga, ua * sua));
+        if constexpr (TWO) r0.y[ia] = f2bf(ds_silu_mul(ga0 * sga, ua0 * sua));
+      }
+      if (ib < g.rows) {
+        act[ib] = f2bf(ds_silu_mul(gb * sgb, ub * sub));
+        if constexpr (TWO) r0.y[ib] = f2bf(ds_silu_mul(gb0 * sgb, ub0 * sub));
+      }
+    }
+  }
+}
+// K > 2048: 2R rows per slot (R = kDsWarps / segs, the bf16 rows per job); warp w owns (row w / segs, segment w % segs)
+// of both R-row groups.  Partial sums meet in shared memory and are summed in segment order, then scaled.
+// res: [2 rows][2 buffers][2 groups][kDsWarps]
+template <bool TWO>
+SSDK_DEVINL void ds_consume_split8(DsRing& ring, const DsGeom& g, float* xs, float* res, __nv_bfloat16* y,
+                                   const DsRow0& r0, const float* scale) {
+  if ((int)blockIdx.x >= g.nj) return;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int R = kDsWarps / g.segs;
+  const int row_in_job = warp / g.segs, seg = warp - row_in_job * g.segs;
+  const int seg_len = g.K / g.segs, steps = seg_len >> 8;
+  float xr[kDsMaxSteps][8];
+  ds_load_x(xs + seg * seg_len, steps, lane, xr);
+  const float* x0 = nullptr;
+  if constexpr (TWO) x0 = ds_row0_x(r0, xs, g.K) + seg * seg_len;
+  const size_t off_a = (size_t)row_in_job * g.K + (size_t)seg * seg_len, off_b = off_a + (size_t)R * g.K;
+  unsigned it = 0;
+  for (int s = (int)blockIdx.x; s < g.nj; s += (int)gridDim.x, ++it) {
+    const int row = s * g.rpj + (int)threadIdx.x;  // the output row of a reducing thread (threadIdx.x < g.rpj)
+    const float sc = ((int)threadIdx.x < g.rpj && row < g.rows) ? scale[row] : 0.f;
+    const uint8_t* st = ds_acquire(ring, 0);
+    const float acc_a = ds_dot_seg8(st + off_a, steps, lane, xr);
+    const float acc_b = ds_dot_seg8(st + off_b, steps, lane, xr);
+    float acc0_a = 0.f, acc0_b = 0.f;
+    if constexpr (TWO) {
+      acc0_a = ds_dot_seg08(st + off_a, steps, lane, x0);
+      acc0_b = ds_dot_seg08(st + off_b, steps, lane, x0);
+    }
+    ds_release(ring, 0, lane);
+    ring.taken += 1u;
+    float* rb = res + (it & 1u) * 2 * kDsWarps;  // double buffered, as in ds_consume_split
+    float* rb0 = rb + 4 * kDsWarps;
+    if (lane == 0) {
+      rb[warp] = acc_a;
+      rb[kDsWarps + warp] = acc_b;
+      if constexpr (TWO) {
+        rb0[warp] = acc0_a;
+        rb0[kDsWarps + warp] = acc0_b;
+      }
+    }
+    ds_sync();
+    if ((int)threadIdx.x < g.rpj && row < g.rows) {
+      const int grp = (int)threadIdx.x / R;
+      const int base = grp * kDsWarps + ((int)threadIdx.x - grp * R) * g.segs;
+      float v = 0.f;
+      for (int q = 0; q < g.segs; ++q) v += rb[base + q];
+      y[row] = f2bf(v * sc);
+      if constexpr (TWO) {
+        float v0 = 0.f;
+        for (int q = 0; q < g.segs; ++q) v0 += rb0[base + q];
+        r0.y[row] = f2bf(v0 * sc);
+      }
+    }
+  }
+}
+
+// two: two rows (row 0 = r0).  FP8: e4m3 weights with the per-row scales `scale`
+template <bool FP8 = false>
+SSDK_DEVINL void ds_consume(DsRing& ring, const DsGeom& g, float* xs, float* res, __nv_bfloat16* y, bool two,
+                            const DsRow0& r0, const float* scale = nullptr) {
+  if constexpr (FP8) {
+    if (g.kind == DS_PLAIN) {
+      if (two) ds_consume_plain8<true>(ring, g, xs, y, r0, scale);
+      else ds_consume_plain8<false>(ring, g, xs, y, r0, scale);
+    } else {
+      if (two) ds_consume_split8<true>(ring, g, xs, res, y, r0, scale);
+      else ds_consume_split8<false>(ring, g, xs, res, y, r0, scale);
+    }
+  } else {
+    if (g.kind == DS_PLAIN) {
+      if (two) ds_consume_plain<false, true>(ring, g, xs, y, nullptr, r0);
+      else ds_consume_plain<false>(ring, g, xs, y, nullptr);
+    } else {
+      if (two) ds_consume_split<true>(ring, g, xs, res, y, r0);
+      else ds_consume_split<false>(ring, g, xs, res, y, r0);
+    }
+  }
+}
+template <bool FP8 = false>
+SSDK_DEVINL void ds_consume_gu(DsRing& ring, const DsGeom& g, float* xs, __nv_bfloat16* act, bool two, const DsRow0& r0,
+                               const float* scale = nullptr) {
+  if constexpr (FP8) {
+    if (two) ds_consume_pair8<true>(ring, g, xs, act, r0, scale);
+    else ds_consume_pair8<false>(ring, g, xs, act, r0, scale);
+  } else {
+    if (two) ds_consume_pair<true>(ring, g, xs, act, r0);
+    else ds_consume_pair<false>(ring, g, xs, act, r0);
+  }
 }
 
 SSDK_DEVINL float ds_block_sum(float v, float* red) {  // all consumer threads get the result
@@ -827,14 +1076,22 @@ SSDK_DEVINL void ds_attention_unit(const DsParams& p, const __nv_bfloat16* vqkv,
 }
 
 
-template <int HD, int GMAX>
+// the row scales of layer l's matrix m (FP8 instance; nullptr in the bf16 one)
+template <bool FP8>
+SSDK_DEVINL const float* ds_scale(const DsParams& p, int l, int m) {
+  if constexpr (FP8) return p.fp8_scale[l][m];
+  else return nullptr;
+}
+
+// FP8: the decoder linears are e4m3 with per-row scales (p.fp8_scale); embedding, lm_head and norms stay bf16
+template <int HD, int GMAX, bool FP8 = false>
 __global__ void __launch_bounds__(kDsThreads, 1) draft_stream_kernel(const __grid_constant__ DsParams p) {
   SSDK_DYN_SMEM(uint8_t, ds_smem);
   SSDK_STATIC_SMEM(uint64_t, full_bar, kDsMaxSlots);
   SSDK_STATIC_SMEM(uint64_t, empty_bar, kDsMaxSlots);
   SSDK_STATIC_SMEM(DsGeom, geom, 5);
   SSDK_STATIC_SMEM(float, red, 32);
-  SSDK_STATIC_SMEM(float, res, 4 * kDsWarps);
+  SSDK_STATIC_SMEM(float, res, (FP8 ? 8 : 4) * kDsWarps);
   SSDK_STATIC_SMEM(ArgMax, ared, 32);
   SSDK_SHARED_VAR(int, tok_s);
   SSDK_SHARED_VAR(int, flag_s);
@@ -845,10 +1102,17 @@ __global__ void __launch_bounds__(kDsThreads, 1) draft_stream_kernel(const __gri
   if (threadIdx.x < kDsBtSmem && (int)threadIdx.x < p.max_blocks) bt_s[threadIdx.x] = p.block_table[threadIdx.x];
   if (threadIdx.x == 0) {
     trace_mark(TR_MISC);
-    ds_geometry(p.d, (p.H + 2 * p.KV) * HD, false, &geom[DS_QKV]);
-    ds_geometry(p.H * HD, p.d, false, &geom[DS_O]);
-    ds_geometry(p.d, p.ffn, true, &geom[DS_GU]);
-    ds_geometry(p.ffn, p.d, false, &geom[DS_DOWN]);
+    if constexpr (FP8) {
+      ds_geometry8(p.d, (p.H + 2 * p.KV) * HD, false, &geom[DS_QKV]);
+      ds_geometry8(p.H * HD, p.d, false, &geom[DS_O]);
+      ds_geometry8(p.d, p.ffn, true, &geom[DS_GU]);
+      ds_geometry8(p.ffn, p.d, false, &geom[DS_DOWN]);
+    } else {
+      ds_geometry(p.d, (p.H + 2 * p.KV) * HD, false, &geom[DS_QKV]);
+      ds_geometry(p.H * HD, p.d, false, &geom[DS_O]);
+      ds_geometry(p.d, p.ffn, true, &geom[DS_GU]);
+      ds_geometry(p.ffn, p.d, false, &geom[DS_DOWN]);
+    }
     ds_geometry(p.d, p.vocab, false, &geom[DS_HEAD]);
     for (int s = 0; s < p.n_slots; ++s) {
       mbar_init(&full_bar[s], 1);           // the producer's arrive.expect_tx + the copy's transaction bytes
@@ -860,7 +1124,7 @@ __global__ void __launch_bounds__(kDsThreads, 1) draft_stream_kernel(const __gri
 
   if (threadIdx.x >= kDsConsumers) {
     // ===================== producer warp: the weight stream never waits for a phase =====================
-    if (threadIdx.x == kDsConsumers) ds_producer(p, geom, ds_smem, full_bar, empty_bar);
+    if (threadIdx.x == kDsConsumers) ds_producer<FP8>(p, geom, ds_smem, full_bar, empty_bar);
     return;
   }
 
@@ -907,7 +1171,8 @@ __global__ void __launch_bounds__(kDsThreads, 1) draft_stream_kernel(const __gri
       }
       cur ^= 1;
       ds_mark(f, 0);
-      ds_consume(ring, geom[DS_QKV], xs, res, p.vec_qkv, two, DsRow0{xs + p.d, nullptr, v0.qkv});
+      ds_consume<FP8>(ring, geom[DS_QKV], xs, res, p.vec_qkv, two, DsRow0{xs + p.d, nullptr, v0.qkv},
+                      ds_scale<FP8>(p, l, DS_QKV));
       ds_mark(f, 1);
       bar.sync();
       ds_mark(f, 2);
@@ -937,7 +1202,7 @@ __global__ void __launch_bounds__(kDsThreads, 1) draft_stream_kernel(const __gri
       ds_mark(f, 4);
       // ---- C: o-proj ----
       ds_load_vec(p.vec_attn, p.H * HD, xs);
-      ds_consume(ring, geom[DS_O], xs, res, p.vec_o, two, DsRow0{nullptr, v0.attn, v0.o});
+      ds_consume<FP8>(ring, geom[DS_O], xs, res, p.vec_o, two, DsRow0{nullptr, v0.attn, v0.o}, ds_scale<FP8>(p, l, DS_O));
       ds_mark(f, 5);
       pre = ds_preload(resid[cur], lw.post_norm, p.d);
       bar.sync();
@@ -947,13 +1212,15 @@ __global__ void __launch_bounds__(kDsThreads, 1) draft_stream_kernel(const __gri
       ds_norm_prologue(p.vec_o, resid[cur], resid[cur ^ 1], lw.post_norm, p.eps, p.d, xs, red, &pre);
       cur ^= 1;
       ds_mark(f, 7);
-      ds_consume_gu(ring, geom[DS_GU], xs, p.vec_act, two, DsRow0{xs + p.d, nullptr, v0.act});
+      ds_consume_gu<FP8>(ring, geom[DS_GU], xs, p.vec_act, two, DsRow0{xs + p.d, nullptr, v0.act},
+                         ds_scale<FP8>(p, l, DS_GU));
       ds_mark(f, 8);
       bar.sync();
       ds_mark(f, 9);
       // ---- E: down-proj ----
       ds_load_vec(p.vec_act, p.ffn, xs);
-      ds_consume(ring, geom[DS_DOWN], xs, res, p.vec_down, two, DsRow0{nullptr, v0.act, v0.down});
+      ds_consume<FP8>(ring, geom[DS_DOWN], xs, res, p.vec_down, two, DsRow0{nullptr, v0.act, v0.down},
+                      ds_scale<FP8>(p, l, DS_DOWN));
       ds_mark(f, 10);
       pre = ds_preload(resid[cur], l + 1 < p.L ? p.layers[l + 1].in_norm : p.final_norm, p.d);
       bar.sync();

@@ -361,6 +361,18 @@ struct ssdk_engine {
 
 static size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
+// the decoder linears of every layer are FP8 (the draft: all of them or none, checked by ssdk_finalize)
+static bool model_linears_fp8(const Model& m) {
+  for (const LayerW& lw : m.layers)
+    if (!lw.qkv.scale || !lw.o.scale || !lw.gate_up.scale || !lw.down.scale) return false;
+  return !m.layers.empty();
+}
+static bool model_any_linear_fp8(const Model& m) {
+  for (const LayerW& lw : m.layers)
+    if (lw.qkv.scale || lw.o.scale || lw.gate_up.scale || lw.down.scale) return true;
+  return false;
+}
+
 static void derive(Model& m) {
   const auto& c = m.cfg;
   m.H = c.heads / c.tp_size;
@@ -963,11 +975,11 @@ static bool use_draft_stream(ssdk_engine* e, int B, int ctx_bound) {
   return drf.present && draft_stream_enabled() && draft_stream_supported(drf, B) &&
          ctx_bound + e->rt.spec_k + 1 <= draft_stream_max_ctx();
 }
-template <int HD, int GMAX>
+template <int HD, int GMAX, bool FP8>
 static int launch_draft_stream(Launcher& L, const DsParams& p, size_t smem) {
   static bool attr_set = false;
   if (!attr_set) {
-    CK(cudaFuncSetAttribute(draft_stream_kernel<HD, GMAX>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CK(cudaFuncSetAttribute(draft_stream_kernel<HD, GMAX, FP8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr_set = true;
   }
   cudaLaunchConfig_t cfg = {};
@@ -980,7 +992,7 @@ static int launch_draft_stream(Launcher& L, const DsParams& p, size_t smem) {
   attr[0].val.cooperative = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;  // (a plain launch measured the same step time: 5.70 vs 5.66 ms — the attribute costs nothing between steps)
-  cudaError_t err = cudaLaunchKernelEx(&cfg, draft_stream_kernel<HD, GMAX>, p);
+  cudaError_t err = cudaLaunchKernelEx(&cfg, draft_stream_kernel<HD, GMAX, FP8>, p);
   if (err != cudaSuccess) return fail("draft stream launch failed: %s", cudaGetErrorString(err));
   L.barrier_op();  // not a PDL primary: the next kernel starts after this grid has drained
   ++L.count;
@@ -1023,13 +1035,21 @@ static int enqueue_draft_stream(ssdk_engine* e, Launcher& L, int64_t* tok_buf, i
   for (int l = 0; l < p.L; ++l) {
     const LayerW& lw = m.layers[l];
     p.layers[l] = DsLayer{lw.qkv.ptr, lw.o.ptr, lw.gate_up.ptr, lw.down.ptr, lw.input_norm, lw.post_norm, lw.q_norm, lw.k_norm};
+    const WeightMat* mats[4] = {&lw.qkv, &lw.o, &lw.gate_up, &lw.down};  // DS_QKV .. DS_DOWN
+    for (int i = 0; i < 4; ++i) p.fp8_scale[l][i] = mats[i]->scale;
   }
   const int G = m.H / m.KV, gmax = G <= 4 ? 4 : 8;
   const size_t smem = ds_fixed_smem(m) + (size_t)p.n_slots * kDsSlotBytes;
-  if (m.hd == 64 && gmax == 4) return launch_draft_stream<64, 4>(L, p, smem);
-  if (m.hd == 64 && gmax == 8) return launch_draft_stream<64, 8>(L, p, smem);
-  if (m.hd == 128 && gmax == 4) return launch_draft_stream<128, 4>(L, p, smem);
-  return launch_draft_stream<128, 8>(L, p, smem);
+  if (model_linears_fp8(m)) {  // every decoder linear is FP8 (ssdk_finalize refuses a mixed draft)
+    if (m.hd == 64 && gmax == 4) return launch_draft_stream<64, 4, true>(L, p, smem);
+    if (m.hd == 64 && gmax == 8) return launch_draft_stream<64, 8, true>(L, p, smem);
+    if (m.hd == 128 && gmax == 4) return launch_draft_stream<128, 4, true>(L, p, smem);
+    return launch_draft_stream<128, 8, true>(L, p, smem);
+  }
+  if (m.hd == 64 && gmax == 4) return launch_draft_stream<64, 4, false>(L, p, smem);
+  if (m.hd == 64 && gmax == 8) return launch_draft_stream<64, 8, false>(L, p, smem);
+  if (m.hd == 128 && gmax == 4) return launch_draft_stream<128, 4, false>(L, p, smem);
+  return launch_draft_stream<128, 8, false>(L, p, smem);
 }
 
 static int enqueue_spec_step(ssdk_engine* e, Launcher& L, int B, bool host_io, bool advance, bool stream_draft) {
@@ -1202,6 +1222,7 @@ int ssdk_create(const ssdk_model_cfg* target, const ssdk_model_cfg* draft, const
   if (rt->max_batch < 1 || rt->max_batch * (rt->spec_k + 1) > kMaxTokens || rt->max_batch > kVerifyMaxBatch)
     return fail("max_batch=%d: need max_batch*(K+1) <= %d and max_batch <= %d", rt->max_batch, kMaxTokens, kVerifyMaxBatch);
   if (rt->spec_k > 0 && !draft && target->tp_rank == 0) return fail("spec_k>0 needs a draft model on rank 0");
+  if (rt->draft_fp8 != 0 && rt->draft_fp8 != 1) return fail("draft_fp8=%d: 0 (bf16 draft) or 1 (FP8 draft)", rt->draft_fp8);
   ssdk_engine* e = new ssdk_engine();
   e->rt = *rt;
   const ssdk_model_cfg* cfgs[2] = {target, draft};
@@ -1313,7 +1334,9 @@ int ssdk_bind_weight(ssdk_handle h, int which, int kind, int layer, const void* 
 int ssdk_bind_weight_fp8(ssdk_handle h, int which, int kind, int layer, const void* w_e4m3, const float* row_scale,
                          int64_t rows, int64_t cols) {
   if (!h || which < 0 || which > 1 || !h->model[which].present) return fail("bind_weight_fp8: bad handle/model");
-  if (which != SSDK_TARGET) return fail("bind_weight_fp8: FP8 weights are supported for the target model only");
+  if (which != SSDK_TARGET && !h->rt.draft_fp8)
+    return fail("bind_weight_fp8: FP8 weights are supported for the target model only unless the runtime config sets "
+                "draft_fp8 = 1");
   if (!w_e4m3 || !row_scale) return fail("bind_weight_fp8: null pointer");
   Model& m = h->model[which];
   if (layer < 0 || layer >= m.cfg.layers) return fail("bind_weight_fp8: layer %d out of range", layer);
@@ -1409,6 +1432,11 @@ int ssdk_finalize(ssdk_handle h, void* stream) {
     }
     CKI(weight_tmap(m.lm_head));
   }
+  // one weight format per draft, so one streaming-kernel instance: draft_fp8 = 1 asks for every decoder linear in FP8
+  const Model& drf = h->model[SSDK_DRAFT];
+  if (drf.present && h->rt.draft_fp8 && !model_linears_fp8(drf))
+    return fail("finalize: draft_fp8 = 1 but the draft's decoder linears are %s: bind qkv, o, gate_up and down of every "
+                "draft layer with ssdk_bind_weight_fp8", model_any_linear_fp8(drf) ? "partly bf16" : "bf16");
   CKI(init_kernel_attrs());
   CK(cudaMemsetAsync(h->ws_base, 0, (size_t)carve(h, nullptr), st));
   CK(cudaStreamSynchronize(st));

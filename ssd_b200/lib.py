@@ -34,7 +34,7 @@ class RuntimeCfg(C.Structure):
     _fields_ = [
         ("spec_k", C.c_int32), ("max_batch", C.c_int32), ("block_size", C.c_int32),
         ("max_blocks_per_seq", C.c_int32), ("use_graph", C.c_int32), ("use_pdl", C.c_int32),
-        ("jit_speculate", C.c_int32), ("reserved", C.c_int32),
+        ("jit_speculate", C.c_int32), ("draft_fp8", C.c_int32),
     ]
 
 

@@ -39,7 +39,7 @@ def load_safetensors_weights(path: str, spec: ModelSpec, device, tp_size: int = 
     packed matrix then gets fp32 per-row scales lw[name + "_scale"] (a per-tensor scale is broadcast to its rows, so
     q|k|v and gate|up with different per-tensor scales become one per-row vector).  `input_scale` / `input_scale_ub`
     are activation scales of W8A8 kernels and are ignored (listed in w["ignored"]).  Block-wise scales
-    (`weight_scale_inv`) raise NotImplementedError, and so does any FP8 tensor when allow_fp8 is False (the draft)."""
+    (`weight_scale_inv`) raise NotImplementedError, and so does any FP8 tensor when allow_fp8 is False."""
     from safetensors import safe_open
 
     H, KV, hd = spec.heads // tp_size, spec.kv_heads // tp_size, spec.head_dim
@@ -106,8 +106,9 @@ def load_safetensors_weights(path: str, spec: ModelSpec, device, tp_size: int = 
                     continue
                 t = f.get_tensor(name)
                 if t.dtype == f8 and not allow_fp8:
-                    raise NotImplementedError(f"{path}: {name} is FP8; FP8 weights are supported for the target model "
-                                              "only (the draft runs in bf16)")
+                    raise NotImplementedError(f"{path}: {name} is FP8 and allow_fp8=False asks for bf16 weights; FP8 "
+                                              "decoder linears load for the draft as well, not for the target model "
+                                              "only: pass allow_fp8=True")
                 parts = name.split(".")
                 if name.startswith("model.layers.") and ".".join(parts[3:-1]) in _LINEAR_LEAVES and \
                         parts[-1] in ("weight", "weight_scale"):
@@ -200,19 +201,20 @@ def tp_row_amax_max(amax: torch.Tensor) -> torch.Tensor:
 
 def load_weights(path: str, spec: ModelSpec, device, tp_size: int = 1, tp_rank: int = 0,
                  quantization: str | None = None, is_target: bool = True) -> dict:
-    """Packed per-rank weights of a synthetic directory or a safetensors checkpoint.  quantization="fp8" (target
-    only) replaces the decoder linears by e4m3 + per-row scales (quant.py) after loading, one tensor at a time; FP8
-    checkpoint tensors are kept as they are either way.  With tp_size > 1 every rank must call this together: the row
-    scales of o / down come from the full rows (a MAX all-reduce over the ranks' column shards)."""
-    if quantization is not None and not is_target:
-        raise NotImplementedError("quantization applies to the target model only (the draft runs in bf16)")
+    """Packed per-rank weights of a synthetic directory or a safetensors checkpoint.  quantization="fp8" replaces the
+    decoder linears by e4m3 + per-row scales (quant.py) after loading, one tensor at a time; FP8 checkpoint tensors are
+    kept as they are either way.  With tp_size > 1 every rank must call this together: the row scales of o / down come
+    from the full rows (a MAX all-reduce over the ranks' column shards).  The draft (is_target=False) is a tp = 1
+    replica on rank 0, so its rows are whole and need no reduction."""
+    if not is_target and tp_size != 1:
+        raise ValueError("the draft is loaded whole (tp_size = 1) on rank 0")
     marker = os.path.join(path, "ssd_b200_synthetic.json")
     if os.path.exists(marker):
         from .synth import generate_weights
         with open(marker) as f:
             w = generate_weights(spec, json.load(f), device, tp_size, tp_rank)
     elif glob.glob(os.path.join(path, "*.safetensors")):
-        w = load_safetensors_weights(path, spec, device, tp_size, tp_rank, allow_fp8=is_target)
+        w = load_safetensors_weights(path, spec, device, tp_size, tp_rank, allow_fp8=True)
     else:
         raise FileNotFoundError(f"{path}: neither *.safetensors nor ssd_b200_synthetic.json")
     if quantization == "fp8":
@@ -221,6 +223,20 @@ def load_weights(path: str, spec: ModelSpec, device, tp_size: int = 1, tp_rank: 
         if torch.device(device).type == "cuda":
             torch.cuda.empty_cache()
     return w
+
+
+def load_draft_weights(config, spec: ModelSpec, device) -> dict:
+    """The draft's packed weights, a whole (tp = 1) replica.  config.draft_quantization="fp8" quantizes its decoder
+    linears on load.  An FP8 draft checkpoint loads as FP8 either way (found by its quantization_config in Config, or
+    here by its e4m3 tensors), and config.draft_quantization then reads "fp8".  A draft runs in one weight format, so a
+    bf16 decoder linear next to FP8 ones is quantized too."""
+    wd = load_weights(config.draft, spec, device, quantization=config.draft_quantization, is_target=False)
+    if is_fp8(wd) and config.draft_quantization is None:
+        config.draft_quantization = "fp8"
+        quantize_layers_(wd)
+        if torch.device(device).type == "cuda":
+            torch.cuda.empty_cache()
+    return wd
 
 
 class _DraftCfg:
@@ -252,7 +268,7 @@ def build_runner(config, tp_size: int = 1, tp_rank: int = 0, device=None, finali
     wt = load_weights(config.model, tspec, device, tp_size, tp_rank, quantization=config.quantization)
     if is_fp8(wt):  # an FP8 checkpoint found by its tensor dtypes
         config.quantization = "fp8"
-    wd = load_weights(config.draft, dspec, device, is_target=False) if (dspec is not None and tp_rank == 0) else None
+    wd = load_draft_weights(config, dspec, device) if (dspec is not None and tp_rank == 0) else None
     if dspec is not None and tp_rank != 0:
         dspec = None  # the draft is a replica pinned to rank 0 (SURVEY §8e)
     nbt = kv_blocks_for(config, tspec, tp_size, 0.8 if dspec else 1.0)
@@ -264,7 +280,7 @@ def build_runner(config, tp_size: int = 1, tp_rank: int = 0, device=None, finali
                         max_batch=max(1, config.max_num_seqs), block_size=config.kvcache_block_size,
                         max_model_len=config.max_model_len, num_blocks_target=nbt, num_blocks_draft=nbd, device=device,
                         use_graph=config.use_cuda_graph, use_pdl=config.use_pdl, jit_speculate=config.jit_speculate,
-                        tp_size=tp_size, tp_rank=tp_rank)
+                        tp_size=tp_size, tp_rank=tp_rank, draft_fp8=wd is not None and is_fp8(wd))
     runner.bind_weights(L.TARGET, wt)
     if wd is not None:
         runner.bind_weights(L.DRAFT, wd)

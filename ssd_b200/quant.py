@@ -1,4 +1,5 @@
-"""FP8 (e4m3fn) weight-only quantization of the target's decoder linears.
+"""FP8 (e4m3fn) weight-only quantization of the decoder linears, of the target (Config.quantization) and of the draft
+(Config.draft_quantization), each independently of the other.
 
 One format, owned here and by ssdk_bind_weight_fp8 (include/ssdk.h): an FP8 matrix is a float8_e4m3fn tensor
 W8 [N, K] in the bf16 matrix's row order plus fp32 per-row scales s [N]; row n stands for s[n] * W8[n, :].
@@ -13,7 +14,7 @@ from __future__ import annotations
 import torch
 
 E4M3_MAX = 448.0
-FP8_LINEARS = ("qkv", "o", "gate_up", "down")  # the target's decoder linears; embedding, lm_head and norms stay bf16
+FP8_LINEARS = ("qkv", "o", "gate_up", "down")  # the decoder linears of either model; embedding, lm_head and norms stay bf16
 
 
 def quantize_fp8_rowwise(w: torch.Tensor, row_amax: torch.Tensor | None = None) -> tuple[torch.Tensor, torch.Tensor]:
@@ -84,4 +85,4 @@ def parse_quantization(q: str | None) -> str | None:
     if q is None or q == "fp8":
         return q
     raise ValueError(f"quantization={q!r}: supported values are None (bf16 weights) and 'fp8' (e4m3 weight-only "
-                     "quantization of the target's decoder linears)")
+                     "quantization of the model's decoder linears)")

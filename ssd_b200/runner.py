@@ -68,7 +68,8 @@ class PairRunner:
     def __init__(self, target: ModelSpec, draft: ModelSpec | None, *, spec_k: int, max_batch: int = 1,
                  block_size: int = 256, max_model_len: int = 4096, num_blocks_target: int | None = None,
                  num_blocks_draft: int | None = None, device: str | torch.device = "cuda:0", use_graph: bool = True,
-                 use_pdl: bool = False, jit_speculate: bool = True, tp_size: int = 1, tp_rank: int = 0):
+                 use_pdl: bool = False, jit_speculate: bool = True, tp_size: int = 1, tp_rank: int = 0,
+                 draft_fp8: bool = False):
         if not torch.cuda.is_available():
             raise RuntimeError("PairRunner needs a CUDA device: libssdk has no CPU path")
         self.lib = L.load()
@@ -89,7 +90,7 @@ class PairRunner:
         tcfg = cfg(target, tp_size, tp_rank)
         dcfg = cfg(draft, 1, 0) if draft is not None else None
         rt = L.RuntimeCfg(spec_k, max_batch, block_size, self.max_blocks, int(use_graph),
-                          int(use_pdl), int(jit_speculate), 0)
+                          int(use_pdl), int(jit_speculate), int(draft_fp8))
         h = C.c_void_p()
         L.check(self.lib.ssdk_create(C.byref(tcfg), C.byref(dcfg) if dcfg is not None else None, C.byref(rt),
                                      C.byref(h)), "ssdk_create")
@@ -126,8 +127,8 @@ class PairRunner:
     def bind_weights(self, which: int, w: dict) -> None:
         """w: packed per-rank tensors on this device (bf16):
         embed, lm_head, final_norm, layers[l] = {input_norm, qkv, o, post_norm, gate_up, down[, q_norm, k_norm]}.
-        A decoder linear of the target may instead be float8_e4m3fn with fp32 row scales in layers[l][name + "_scale"]
-        (quant.py); it is bound with ssdk_bind_weight_fp8."""
+        A decoder linear may instead be float8_e4m3fn with fp32 row scales in layers[l][name + "_scale"] (quant.py); it
+        is bound with ssdk_bind_weight_fp8.  A draft with FP8 linears needs draft_fp8=True, and then all of them."""
         lib, h = self.lib, self.h
 
         def bind(kind, layer, t, scale=None):

@@ -9,7 +9,13 @@
            tokens of both loops against the closed-form greedy chain of the synthetic target.
   prefill  the same pair prefilled (target + draft): 16 x 128-token prompts through prefill_many and the ragged set of
            tools/bench_prefill.py through prefill_many and prefill_varlen; median of three alternated warm runs.
-    python tools/bench_fp8.py [--sections gemm,e2e,prefill] [--m 1,7,16,64,256] [--out OUT.json]"""
+  draft    the e2e workload in four configurations, target / draft = bf16 / bf16, bf16 / FP8, FP8 / bf16 and FP8 / FP8
+           (quantization, draft_quantization), all resident in one process and alternated, 3 runs each after a warm-up
+           round: `value` and `e2e` tok/s, accept-len, chain mismatches, the draft phase's device time per step (the
+           streaming draft kernel, from torch.profiler over 16 resident steps) with the GB/s that implies over the draft's
+           weight bytes per step (computed from its shapes, not measured), and the step time with a 3000-token prompt,
+           where the draft runs kernel-per-op (as tools/check_draft_stream.py --prompt-len 3000).
+    python tools/bench_fp8.py [--sections gemm,e2e,prefill,draft] [--m 1,7,16,64,256] [--out OUT.json]"""
 import argparse
 import atexit
 import gc
@@ -92,13 +98,13 @@ def _close(llm) -> None:
     torch.cuda.empty_cache()
 
 
-def _pair(root, quantization, **kw):
+def _pair(root, quantization, draft_quantization=None, **kw):
     from ssd_b200 import synth
     from ssd_b200.llm import LLM
     t = synth.make_model_dir(root, "llama-3.1-8b", "target", seed=0)
     d = synth.make_model_dir(root, "llama-3.2-1b", "draft", seed=0)
     return LLM(t, speculate=True, draft=d, speculate_k=6, num_gpus=1, kvcache_block_size=256, jit_speculate=True,
-               quantization=quantization, **kw)
+               quantization=quantization, draft_quantization=draft_quantization, **kw)
 
 
 def _run_once(llm, prompt, steps, warm):
@@ -179,6 +185,101 @@ def bench_e2e(a, out):
         _close(llm)
 
 
+def _resident(llm, prompt, warm):
+    from ssd_b200 import lib as L
+    r = llm.runner
+    bt = list(range(r.max_blocks))
+    rec = r.prefill(L.TARGET, prompt, bt)
+    r.prefill(L.DRAFT, prompt, bt, want_sample=False)
+    r.stage([len(prompt)], [rec], [bt], [bt], [0.0], [0.0])
+    for _ in range(warm):
+        r.step_resident(1)
+    torch.cuda.synchronize()
+    return r
+
+
+def _draft_phase_ms(llm, prompt, steps=16):
+    """Device time per step of the streaming draft kernel (the whole draft phase at this shape), by torch.profiler."""
+    from torch.profiler import ProfilerActivity, profile
+    r = _resident(llm, prompt, 4)
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(steps):
+            r.step_resident(1)
+        torch.cuda.synchronize()
+    us = sum(getattr(e, "device_time_total", getattr(e, "cuda_time_total", 0)) for e in prof.key_averages()
+             if "draft_stream_kernel" in e.key)
+    return us / 1e3 / steps if us else None
+
+
+def _step_ms(llm, prompt, steps=16):
+    r = _resident(llm, prompt, 4)
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(steps):
+        r.step_resident(1)
+    e1.record()
+    torch.cuda.synchronize()
+    return e0.elapsed_time(e1) / steps
+
+
+def _draft_bytes_per_step(llm) -> dict:
+    """Weight bytes the K draft forwards of one step stream (arithmetic from the shapes): decoder linears at 2 B (bf16)
+    or 1 B + 4 B per row scale (FP8), plus the bf16 lm_head."""
+    h, k = llm.config.draft_hf_config, llm.config.speculate_k
+    d, hd, ffn = h.hidden_size, h.head_dim, h.intermediate_size
+    qkv = (h.num_attention_heads + 2 * h.num_key_value_heads) * hd
+    weights = qkv * d + d * h.num_attention_heads * hd + 2 * ffn * d + d * ffn
+    rows = qkv + d + 2 * ffn + d
+    head = h.vocab_size * d * 2
+    return {"bf16": k * (h.num_hidden_layers * weights * 2 + head),
+            "fp8": k * (h.num_hidden_layers * (weights + 4 * rows) + head)}
+
+
+def bench_draft(a, out):
+    from ssd_b200 import synth
+    root = tempfile.mkdtemp(prefix="ssd_b200_fp8_")
+    pi_t = synth.permutations(synth.SHAPES["llama-3.1-8b"][6], 0, 0.85, "cpu")[0].tolist()
+
+    def mismatches(prompt, toks):
+        bad, prev = 0, prompt[-1]
+        for t in toks:
+            bad += int(t != pi_t[prev])
+            prev = t
+        return bad
+
+    configs = {"bf16/bf16": (None, None), "bf16/fp8": (None, "fp8"), "fp8/bf16": ("fp8", None), "fp8/fp8": ("fp8", "fp8")}
+    llms = {k: _pair(root, q, dq, max_num_seqs=1, max_model_len=4096) for k, (q, dq) in configs.items()}
+    nbytes = _draft_bytes_per_step(next(iter(llms.values())))
+    res = {k: [] for k in llms}
+    for rep in range(4):  # alternated; round 0 is a warm-up
+        rng = random.Random(100 + rep)
+        prompt = [rng.randint(0, 10000) for _ in range(128)]
+        long_prompt = [rng.randint(0, 10000) for _ in range(3000)]
+        for k, llm in llms.items():
+            v, e, acc, dlog, elog = _run_once(llm, prompt, a.steps, 8)
+            dms = _draft_phase_ms(llm, prompt)
+            lms = _step_ms(llm, long_prompt)
+            if rep:
+                res[k].append({"value": v, "e2e": e, "accept_len": acc, "tokens": len(dlog) + len(elog),
+                               "chain_mismatches": mismatches(prompt, dlog) + mismatches(prompt, elog),
+                               "draft_ms_per_step": dms, "step_ms_prompt3000": lms})
+    for k, runs in res.items():
+        fmt = "fp8" if configs[k][1] else "bf16"
+        rec = {"section": "draft", "target/draft": k, "draft_GB_per_step": round(nbytes[fmt] / 1e9, 2),
+               "runs": [{kk: round(vv, 3) if isinstance(vv, float) else vv for kk, vv in r_.items()} for r_ in runs]}
+        for m in ("value", "e2e", "accept_len", "draft_ms_per_step", "step_ms_prompt3000"):
+            xs = sorted(r_[m] for r_ in runs if r_[m] is not None)
+            if xs:
+                rec[m] = {"median": round(xs[len(xs) // 2], 3), "min": round(xs[0], 3), "max": round(xs[-1], 3)}
+        rec["chain_mismatches"] = sum(r_["chain_mismatches"] for r_ in runs)
+        if "draft_ms_per_step" in rec:
+            rec["draft_GBps_implied"] = round(nbytes[fmt] / (rec["draft_ms_per_step"]["median"] * 1e6), 1)
+        print(json.dumps(rec), flush=True)
+        out.append(rec)
+    for llm in llms.values():
+        _close(llm)
+
+
 def bench_prefill(a, out):
     from ssd_b200 import lib as L
     root = tempfile.mkdtemp(prefix="ssd_b200_fp8_")
@@ -238,7 +339,7 @@ def main():
     out = [card()]
     print(json.dumps(out[0]), flush=True)
     for sec in a.sections.split(","):
-        {"gemm": bench_gemm, "e2e": bench_e2e, "prefill": bench_prefill}[sec](a, out)
+        {"gemm": bench_gemm, "e2e": bench_e2e, "prefill": bench_prefill, "draft": bench_draft}[sec](a, out)
     if a.out:
         with open(a.out, "w") as f:
             json.dump(out, f, indent=1)
