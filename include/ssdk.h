@@ -118,6 +118,16 @@ int ssdk_bind_weight_fp8(ssdk_handle h, int which, int kind, int layer,
  * k = base, v = base + L*num_blocks*block_size*kv_heads/tp*hd elements. */
 int ssdk_bind_kv_cache(ssdk_handle h, int which, void* kv_base, int64_t num_blocks);
 
+/* FP8 KV cache, called instead of ssdk_bind_kv_cache and before ssdk_finalize;
+ * the reference has no FP8 KV path.  which: SSDK_TARGET only (the draft's cache
+ * stays bf16).  Same [2, L, num_blocks, block_size, kv_heads/tp, hd] layout with
+ * float8 e4m3fn elements (one byte each), 16-byte aligned; head_dim 64 or 128.
+ * k_scale, v_scale: host fp32 arrays [L], finite and > 0, copied into the handle.
+ * Layer l stores code = e4m3_rne(sat448(y / s)) of the bf16 value y the bf16
+ * cache would hold, and attention reads K = k_scale[l] * code, V = v_scale[l] * code. */
+int ssdk_bind_kv_cache_fp8(ssdk_handle h, int which, void* kv_base, int64_t num_blocks,
+                           const float* k_scale, const float* v_scale);
+
 /* Scratch owned by the caller (activations, split-K partials, attention partials,
  * logits_q/logits_p, token buffers). */
 int64_t ssdk_workspace_bytes(ssdk_handle h);
@@ -269,6 +279,15 @@ int ssdk_rope_store_kv(const void* qkv, const int64_t* positions, const int32_t*
                        const float* rope_table, const void* q_norm_w, const void* k_norm_w,
                        float norm_eps, void* q_out, void* k_cache, void* v_cache,
                        int M, int heads, int kv_heads, int head_dim, void* stream);
+/* ssdk_rope_store_kv into e4m3 caches (layout of ssdk_bind_kv_cache_fp8, one byte
+ * per element; head_dim 64 or 128): k and v are stored as
+ * e4m3_rne(sat448(y / scale)) of the bf16 values y the bf16 op stores; q_out as
+ * in the bf16 op.  The reference has no FP8 KV path. */
+int ssdk_rope_store_kv_fp8(const void* qkv, const int64_t* positions, const int32_t* slot_mapping,
+                           const float* rope_table, const void* q_norm_w, const void* k_norm_w,
+                           float norm_eps, void* q_out, void* k_cache, void* v_cache,
+                           int M, int heads, int kv_heads, int head_dim,
+                           float k_scale, float v_scale, void* stream);
 
 /* silu(x[:, :ffn]) * x[:, ffn:]  (layers/activation.py:11-14). */
 int ssdk_silu_mul(const void* gate_up, void* out, int M, int ffn, void* stream);
@@ -300,6 +319,22 @@ int ssdk_paged_attn_varlen(const void* q, const void* k_cache, const void* v_cac
 /* Its plan: out5 = {TQ, MT, n_qtiles of the longest sequence, n_split, tiles in the launch}.
  * With every q_lens[b] equal the first four are ssdk_paged_attn_plan's. */
 int ssdk_paged_attn_varlen_plan(int heads, int kv_heads, int batch, const int32_t* q_lens, int max_ctx, int* out5);
+/* ssdk_paged_attn and ssdk_paged_attn_varlen over e4m3 caches (layout of
+ * ssdk_bind_kv_cache_fp8): attention over K = k_scale * code, V = v_scale * code,
+ * q and out bf16, the same plans and scratch sizes as the bf16 ops.  The
+ * reference has no FP8 KV path. */
+int ssdk_paged_attn_fp8(const void* q, const void* k_cache, const void* v_cache,
+                        const int32_t* block_tables, const int32_t* context_lens,
+                        void* out, void* scratch,
+                        int batch, int q_len, int heads, int kv_heads, int head_dim,
+                        int block_size, int max_blocks_per_seq, float scale,
+                        float k_scale, float v_scale, void* stream);
+int ssdk_paged_attn_varlen_fp8(const void* q, const void* k_cache, const void* v_cache,
+                               const int32_t* block_tables, const int32_t* context_lens,
+                               const int32_t* q_lens, void* out, void* scratch,
+                               int batch, int heads, int kv_heads, int head_dim,
+                               int block_size, int max_blocks_per_seq, float scale,
+                               float k_scale, float v_scale, void* stream);
 
 /* Sampler.forward (layers/sampler.py:14-36): greedy where temp==0, else
  * argmax(softmax(l/T) / Exp(1)) with Philox(seed, step_id) exponentials.

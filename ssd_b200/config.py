@@ -8,7 +8,7 @@ import os
 from dataclasses import dataclass
 
 from .paths import DEFAULT_DRAFT, DEFAULT_TARGET
-from .quant import checkpoint_quantization, parse_quantization
+from .quant import checkpoint_quantization, parse_kv_cache_dtype, parse_quantization
 
 
 @dataclass
@@ -59,6 +59,11 @@ class Config:
     # draft changes only the acceptance rate and the speed.  An FP8 draft checkpoint is loaded as FP8 whatever this says,
     # and the field then reads "fp8".
     draft_quantization: str | None = None
+    # "fp8" (or "fp8_e4m3"): the TARGET's KV cache is stored as float8 e4m3 with one fp32 scale per layer for K and one
+    # for V (the checkpoint's self_attn.k_scale / v_scale, else 1.0; DESIGN.md §3).  Half the bytes per token, twice the
+    # pages in the same memory.  This changes the outputs.  The draft's cache stays bf16.  "auto" (or "bf16",
+    # "bfloat16"): bf16, the default; the field then reads "auto".
+    kv_cache_dtype: str = "auto"
 
     @property
     def max_blocks(self) -> int:
@@ -77,6 +82,7 @@ class Config:
             self.use_cuda_graph = False
         self.quantization = parse_quantization(self.quantization)
         self.draft_quantization = parse_quantization(self.draft_quantization)
+        self.kv_cache_dtype = parse_kv_cache_dtype(self.kv_cache_dtype)
         self.hf_config = load_hf_config(self.model)
         if checkpoint_quantization(self.hf_config) == "fp8":
             self.quantization = "fp8"

@@ -132,7 +132,8 @@ struct AttnParams {
   float* part_lse;               // [B*Q*H, n_split]
   int B, Q, H, KV, block_size, max_blocks, n_split, TQ, n_qtiles;
   int g_shift;                   // log2(H / KV) when the GQA ratio is a power of two, else -1
-  float scale_log2;              // softmax scale * log2(e)
+  float scale_log2;              // softmax scale * log2(e)  (KV8: * k_scale)
+  float v_scale;                 // KV8 only: V = v_scale * code, applied with the final 1 / l
 };
 
 #ifndef SSDK_HOST_EMU
@@ -170,9 +171,32 @@ SSDK_DEVINL uint32_t pack_bf16x2(float lo, float hi) {
   return *reinterpret_cast<uint32_t*>(&v);
 }
 
+// Dynamic shared memory of one CTA, either cache dtype: two stages of bf16 K and V chunks, which the epilogue's
+// NW * 16 * (HD + 8) fp32 merge buffer reuses.
+constexpr int attn_smem_bytes(int HD) { return 2 * 2 * kAttChunk * (HD + 8) * 2; }
+
+// 16 e4m3 codes -> 16 bf16 (exact: every e4m3 value is a bf16 value)
+SSDK_DEVINL void attn_widen_e4m3x16(const uint8_t* src, __nv_bfloat16* dst) {
+  const uint4 w = *reinterpret_cast<const uint4*>(src);
+  const uint32_t c[4] = {w.x, w.y, w.z, w.w};
+  uint32_t o[8];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const float2 a = e4m3x2_to_float2(c[i]), b = e4m3x2_to_float2(c[i] >> 16);
+    o[2 * i] = pack_bf16x2(a.x, a.y);
+    o[2 * i + 1] = pack_bf16x2(b.x, b.y);
+  }
+  reinterpret_cast<uint4*>(dst)[0] = make_uint4(o[0], o[1], o[2], o[3]);
+  reinterpret_cast<uint4*>(dst)[1] = make_uint4(o[4], o[5], o[6], o[7]);
+}
+
 // One CTA: kv head blockIdx.x, split blockIdx.y, query tile blockIdx.z (of a uniform launch, or an entry of the varlen
 // tile table).
-template <int HD, int MT, bool VARLEN>
+// KV8: the caches hold float8 e4m3 codes (HD bytes per (token, kv head) row) with K = k_scale * code (folded into
+// p.scale_log2) and V = v_scale * code (p.v_scale, applied with the final 1 / l).  The raw chunks are staged with 16-byte
+// cp.async, double buffered, in the upper part of the bf16 instance's shared memory; each chunk is widened (exactly) into
+// one bf16 K/V buffer laid out as a bf16 stage, and the ldmatrix / mma path below is the bf16 one.
+template <int HD, int MT, bool VARLEN, bool KV8>
 SSDK_DEVINL void paged_attn_cta(const AttnParams& p, const AttnVarlen& v) {
   constexpr int NW = attn_warps(MT);
   constexpr int kAttThreads = NW * 32;
@@ -182,11 +206,14 @@ SSDK_DEVINL void paged_attn_cta(const AttnParams& p, const AttnVarlen& v) {
   constexpr int NT = TW / 8;                // 8-token score tiles per warp
   constexpr int KS = HD / 16;               // k-steps over head_dim
   constexpr int ND = HD / 8;                // 8-wide output tiles over head_dim
-  constexpr int SEG = HD / 8;               // 16-byte segments per K/V row
+  constexpr int SEG = KV8 ? HD / 16 : HD / 8;  // 16-byte segments per K/V row
 
   SSDK_DYN_SMEM(uint8_t, att_smem);
-  __nv_bfloat16* sK = reinterpret_cast<__nv_bfloat16*>(att_smem);            // [2][64][LDS]
-  __nv_bfloat16* sV = sK + 2 * kAttChunk * LDS;                              // [2][64][LDS]
+  __nv_bfloat16* sK = reinterpret_cast<__nv_bfloat16*>(att_smem);            // [2][64][LDS]  (KV8: [64][LDS])
+  __nv_bfloat16* sV = sK + (KV8 ? 1 : 2) * kAttChunk * LDS;                  // [2][64][LDS]  (KV8: [64][LDS])
+  // KV8: raw stages [2][K | V][64][HD] bytes after the widened buffers (2 * 64 * (2 HD + 8) * 2 B <= attn_smem_bytes)
+  uint8_t* sRaw = att_smem + 2 * kAttChunk * LDS * 2;
+  static_assert(!KV8 || 2 * kAttChunk * LDS * 2 + 2 * 2 * kAttChunk * HD <= attn_smem_bytes(HD), "KV8 smem");
 
   pdl_launch_dependents();
   pdl_wait();
@@ -252,6 +279,7 @@ SSDK_DEVINL void paged_attn_cta(const AttnParams& p, const AttnVarlen& v) {
     const int base = ch * kAttChunk;
     __nv_bfloat16* dk = sK + stage * kAttChunk * LDS;
     __nv_bfloat16* dv = sV + stage * kAttChunk * LDS;
+    uint8_t* rk = sRaw + stage * 2 * kAttChunk * HD;  // KV8: raw K, then raw V
     int chunk_blk = -1, chunk_off = 0;
     if (page_aligned) {
       chunk_blk = bt[base / p.block_size];
@@ -273,10 +301,24 @@ SSDK_DEVINL void paged_attn_cta(const AttnParams& p, const AttnVarlen& v) {
           in_blk = pos % p.block_size;
         }
         valid = blk >= 0;
-        off = (((size_t)blk * p.block_size + in_blk) * p.KV + kvh) * HD + seg * 8;
+        off = (((size_t)blk * p.block_size + in_blk) * p.KV + kvh) * HD + seg * (KV8 ? 16 : 8);
       }
-      cp_async16(dk + tok * LDS + seg * 8, p.k_cache + off, valid);
-      cp_async16(dv + tok * LDS + seg * 8, p.v_cache + off, valid);
+      if constexpr (KV8) {
+        cp_async16(rk + tok * HD + seg * 16, reinterpret_cast<const uint8_t*>(p.k_cache) + off, valid);
+        cp_async16(rk + kAttChunk * HD + tok * HD + seg * 16, reinterpret_cast<const uint8_t*>(p.v_cache) + off, valid);
+      } else {
+        cp_async16(dk + tok * LDS + seg * 8, p.k_cache + off, valid);
+        cp_async16(dv + tok * LDS + seg * 8, p.v_cache + off, valid);
+      }
+    }
+  };
+  // KV8: widen raw stage `stage` into the bf16 K/V buffers
+  auto widen_chunk = [&](int stage) {
+    const uint8_t* rk = sRaw + stage * 2 * kAttChunk * HD;
+    for (int idx = threadIdx.x; idx < kAttChunk * SEG; idx += kAttThreads) {
+      const int tok = idx / SEG, seg = idx - tok * SEG;
+      attn_widen_e4m3x16(rk + tok * HD + seg * 16, sK + tok * LDS + seg * 16);
+      attn_widen_e4m3x16(rk + kAttChunk * HD + tok * HD + seg * 16, sV + tok * LDS + seg * 16);
     }
   };
 
@@ -291,9 +333,13 @@ SSDK_DEVINL void paged_attn_cta(const AttnParams& p, const AttnVarlen& v) {
       cp_async_wait<1>();
       __syncthreads();
       if (threadIdx.x == 0 && ch == ch_begin) trace_fine(TRF_ATTN + 1);  // first chunk landed
+      if constexpr (KV8) {
+        widen_chunk(stage);
+        __syncthreads();
+      }
 
-      const __nv_bfloat16* cK = sK + stage * kAttChunk * LDS;
-      const __nv_bfloat16* cV = sV + stage * kAttChunk * LDS;
+      const __nv_bfloat16* cK = sK + (KV8 ? 0 : stage) * kAttChunk * LDS;
+      const __nv_bfloat16* cV = sV + (KV8 ? 0 : stage) * kAttChunk * LDS;
       const int tok0 = tslice * TW;
 
       // ---- S = Q K^T ----
@@ -429,7 +475,7 @@ SSDK_DEVINL void paged_attn_cta(const AttnParams& p, const AttnVarlen& v) {
     const int rt = (p.g_shift >= 0) ? (r >> p.g_shift) : r / G;  // token inside the tile; r - rt * G = head of the group
     const int row_q = (VARLEN ? v.cu_q[b] : b * p.Q) + qt * p.TQ + rt;
     const int head = kvh * G + (r - rt * G);
-    const float inv = (l > 0.f) ? 1.f / l : 0.f;
+    const float inv = (l > 0.f) ? (KV8 ? p.v_scale / l : 1.f / l) : 0.f;
     acc.x *= inv; acc.y *= inv; acc.z *= inv; acc.w *= inv;
     if (p.n_split == 1) {
       __nv_bfloat16* dst = p.out + ((size_t)row_q * p.H + head) * HD + d;
@@ -444,14 +490,15 @@ SSDK_DEVINL void paged_attn_cta(const AttnParams& p, const AttnVarlen& v) {
   if (threadIdx.x == 0) trace_fine(TRF_ATTN + 3);  // partials / output stored
 }
 
-template <int HD, int MT>
+// KV8: the caches hold e4m3 codes (see paged_attn_cta)
+template <int HD, int MT, bool KV8 = false>
 __global__ void __launch_bounds__(attn_warps(MT) * 32) paged_attn_kernel(AttnParams p) {
-  paged_attn_cta<HD, MT, false>(p, AttnVarlen{});
+  paged_attn_cta<HD, MT, false, KV8>(p, AttnVarlen{});
 }
 // p.B sequences packed by v.cu_q, grid.z = the tile table's length; p.Q and p.n_qtiles are unused
-template <int HD, int MT>
+template <int HD, int MT, bool KV8 = false>
 __global__ void __launch_bounds__(attn_warps(MT) * 32) paged_attn_varlen_kernel(AttnParams p, AttnVarlen v) {
-  paged_attn_cta<HD, MT, true>(p, v);
+  paged_attn_cta<HD, MT, true, KV8>(p, v);
 }
 
 // Sequence of packed row `tok` of a varlen launch: the b with cu_q[b] <= tok < cu_q[b + 1].

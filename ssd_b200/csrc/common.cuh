@@ -50,6 +50,50 @@ SSDK_DEVINL uint4 pack_bf16x8(const float* f) {
 }
 
 // ----------------------------------------------------------------------------------
+// float8 e4m3fn codes (FP8 draft weights, FP8 KV cache)
+// ----------------------------------------------------------------------------------
+// the two e4m3 codes in the low 16 bits of v (the lower byte is the first) -> two floats, exactly: e4m3 -> f16 is exact
+// (every e4m3 subnormal is an f16 normal), and so is f16 -> f32
+SSDK_DEVINL float2 e4m3x2_to_float2(uint32_t v) {
+#ifdef SSDK_HOST_EMU
+  auto one = [](uint32_t b) {
+    const int e = (int)((b >> 3) & 15u), m = (int)(b & 7u);
+    float x = (e == 15 && m == 7) ? NAN : (e ? std::ldexp(1.0f + (float)m / 8.0f, e - 7) : std::ldexp((float)m, -9));
+    return (b & 0x80u) ? -x : x;
+  };
+  return make_float2(one(v & 0xFFu), one((v >> 8) & 0xFFu));
+#else
+  uint32_t h2;
+  asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(h2) : "h"((unsigned short)(v & 0xFFFFu)));
+  return make_float2(__half2float(__ushort_as_half((unsigned short)(h2 & 0xFFFFu))),
+                     __half2float(__ushort_as_half((unsigned short)(h2 >> 16))));
+#endif
+}
+// two floats -> two e4m3 codes (lo in the lower byte): round to nearest even, finite values saturate to +-448, NaN stays
+// NaN (cvt.rn.satfinite)
+SSDK_DEVINL uint16_t float2_to_e4m3x2(float lo, float hi) {
+#ifdef SSDK_HOST_EMU
+  auto one = [](float x) -> uint32_t {
+    const uint32_t sign = std::signbit(x) ? 0x80u : 0u;
+    const float a = std::fabs(x);
+    if (std::isnan(x)) return sign | 0x7Fu;
+    if (a >= 448.0f) return sign | 0x7Eu;
+    if (a < 0.015625f) return sign | (uint32_t)std::nearbyint(a * 512.0f);  // subnormal steps of 2^-9 (8 -> 2^-6)
+    int e;
+    std::frexp(a, &e);  // a in [2^(e-1), 2^e)
+    int E = e - 1, q = (int)std::nearbyint(std::ldexp(a, 3 - E));  // 8 .. 16 eighths
+    if (q == 16) { q = 8; ++E; }
+    return sign | (uint32_t)((E + 7) << 3) | (uint32_t)(q - 8);
+  };
+  return (uint16_t)(one(lo) | (one(hi) << 8));
+#else
+  uint16_t r;
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(hi), "f"(lo));
+  return r;
+#endif
+}
+
+// ----------------------------------------------------------------------------------
 // warp / block reductions
 // ----------------------------------------------------------------------------------
 SSDK_DEVINL float warp_sum(float v) {

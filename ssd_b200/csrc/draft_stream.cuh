@@ -342,23 +342,6 @@ SSDK_DEVINL float ds_dot_seg(const uint8_t* wseg, int steps, int lane, const flo
   return warp_sum((a0 + a1) + (a2 + a3));
 }
 
-// the two e4m3 codes in the low 16 bits of v (the lower byte is the first) -> two floats, exactly: e4m3 -> f16 is exact
-// (every e4m3 subnormal is an f16 normal), and so is f16 -> f32
-SSDK_DEVINL float2 ds_e4m3x2(uint32_t v) {
-#ifdef SSDK_HOST_EMU
-  auto one = [](uint32_t b) {
-    const int e = (int)((b >> 3) & 15u), m = (int)(b & 7u);
-    float x = (e == 15 && m == 7) ? NAN : (e ? std::ldexp(1.0f + (float)m / 8.0f, e - 7) : std::ldexp((float)m, -9));
-    return (b & 0x80u) ? -x : x;
-  };
-  return make_float2(one(v & 0xFFu), one((v >> 8) & 0xFFu));
-#else
-  uint32_t h2;
-  asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(h2) : "h"((unsigned short)(v & 0xFFFFu)));
-  return make_float2(__half2float(__ushort_as_half((unsigned short)(h2 & 0xFFFFu))),
-                     __half2float(__ushort_as_half((unsigned short)(h2 >> 16))));
-#endif
-}
 // ds_dot_seg for an e4m3 row segment: 8 bytes (the same 8 columns) per lane per step, the same summation order; the
 // caller applies the row scale
 SSDK_DEVINL float ds_dot_seg8(const uint8_t* wseg, int steps, int lane, const float (&xr)[kDsMaxSteps][8]) {
@@ -368,13 +351,13 @@ SSDK_DEVINL float ds_dot_seg8(const uint8_t* wseg, int steps, int lane, const fl
   for (int j = 0; j < kDsMaxSteps; ++j) {
     if (j < steps) {
       const uint2 w = wp[j * 32];
-      float2 f = ds_e4m3x2(w.x);
+      float2 f = e4m3x2_to_float2(w.x);
       a0 = fmaf(f.x, xr[j][0], a0); a1 = fmaf(f.y, xr[j][1], a1);
-      f = ds_e4m3x2(w.x >> 16);
+      f = e4m3x2_to_float2(w.x >> 16);
       a2 = fmaf(f.x, xr[j][2], a2); a3 = fmaf(f.y, xr[j][3], a3);
-      f = ds_e4m3x2(w.y);
+      f = e4m3x2_to_float2(w.y);
       a0 = fmaf(f.x, xr[j][4], a0); a1 = fmaf(f.y, xr[j][5], a1);
-      f = ds_e4m3x2(w.y >> 16);
+      f = e4m3x2_to_float2(w.y >> 16);
       a2 = fmaf(f.x, xr[j][6], a2); a3 = fmaf(f.y, xr[j][7], a3);
     }
   }
@@ -432,13 +415,13 @@ SSDK_DEVINL float ds_dot_seg08(const uint8_t* wseg, int steps, int lane, const f
     const float4 u = *reinterpret_cast<const float4*>(x0 + j * 256 + lane * 8);
     const float4 v = *reinterpret_cast<const float4*>(x0 + j * 256 + lane * 8 + 4);
     const uint2 w = wp[j * 32];
-    float2 f = ds_e4m3x2(w.x);
+    float2 f = e4m3x2_to_float2(w.x);
     a0 = fmaf(f.x, u.x, a0); a1 = fmaf(f.y, u.y, a1);
-    f = ds_e4m3x2(w.x >> 16);
+    f = e4m3x2_to_float2(w.x >> 16);
     a2 = fmaf(f.x, u.z, a2); a3 = fmaf(f.y, u.w, a3);
-    f = ds_e4m3x2(w.y);
+    f = e4m3x2_to_float2(w.y);
     a0 = fmaf(f.x, v.x, a0); a1 = fmaf(f.y, v.y, a1);
-    f = ds_e4m3x2(w.y >> 16);
+    f = e4m3x2_to_float2(w.y >> 16);
     a2 = fmaf(f.x, v.z, a2); a3 = fmaf(f.y, v.w, a3);
   }
   return warp_sum((a0 + a1) + (a2 + a3));

@@ -445,14 +445,21 @@ struct RopeParams {
   const __nv_bfloat16* k_norm_w;
   float norm_eps;
   __nv_bfloat16* q_out;    // [M, H*hd]
-  __nv_bfloat16* k_cache;  // [slots, KV*hd]
+  __nv_bfloat16* k_cache;  // [slots, KV*hd]  (KV8: e4m3 codes, one byte per element)
   __nv_bfloat16* v_cache;
   int heads, kv_heads, head_dim;
+  float k_scale, v_scale;  // KV8 only: the layer's cache scales
 };
+
+// KV8: one k or v element pair, code = e4m3_rne(sat(y / s)) of the bf16 value y the bf16 instance stores (IEEE division)
+SSDK_DEVINL void store_kv8_pair(uint8_t* dst, float a, float b, float s) {
+  *reinterpret_cast<uint16_t*>(dst) = float2_to_e4m3x2(bf16_round(a) / s, bf16_round(b) / s);
+}
 
 // HD is a template parameter so that the per-lane element pairs are static registers (a run-time head_dim turned the
 // x1/x2 arrays into local memory and made ptxas recycle the load registers, i.e. one L2 round trip per split-K slab).
-template <int HD>
+// KV8: k and v go to the cache as e4m3 codes (store_kv8_pair); q is stored as in the bf16 instance.
+template <int HD, bool KV8 = false>
 __global__ void __launch_bounds__(128) rope_store_kernel(RopeParams p) {
   constexpr int HALF = HD / 2;
   constexpr int NP = (HALF + 63) / 64;  // (i, i+1) / (i + HALF, i + HALF + 1) pairs per lane, i = 2 * lane + 64 * t
@@ -484,6 +491,18 @@ __global__ void __launch_bounds__(128) rope_store_kernel(RopeParams p) {
     }
   }
   if (kind != 0 && slot < 0) return;
+  if (kind == 2 && KV8) {
+    uint8_t* dst = reinterpret_cast<uint8_t*>(p.v_cache) + ((size_t)slot * KV + (head - H - KV)) * HD;
+#pragma unroll
+    for (int t = 0; t < NP; ++t) {
+      const int i = 2 * lane + 64 * t;
+      if (i < HALF) {
+        store_kv8_pair(dst + i, x1[t][0], x1[t][1], p.v_scale);
+        store_kv8_pair(dst + HALF + i, x2[t][0], x2[t][1], p.v_scale);
+      }
+    }
+    return;
+  }
   if (kind == 2) {
     __nv_bfloat16* dst = p.v_cache + ((size_t)slot * KV + (head - H - KV)) * HD;
 #pragma unroll
@@ -514,6 +533,20 @@ __global__ void __launch_bounds__(128) rope_store_kernel(RopeParams p) {
     }
   }
   const float* cs = p.rope_table + (size_t)pos * HD;
+  if (KV8 && kind == 1) {
+    uint8_t* dst = reinterpret_cast<uint8_t*>(p.k_cache) + ((size_t)slot * KV + (head - H)) * HD;
+#pragma unroll
+    for (int t = 0; t < NP; ++t) {
+      const int i = 2 * lane + 64 * t;
+      if (i < HALF) {
+        const float2 c = *reinterpret_cast<const float2*>(cs + i), sn = *reinterpret_cast<const float2*>(cs + HALF + i);
+        store_kv8_pair(dst + i, x1[t][0] * c.x - x2[t][0] * sn.x, x1[t][1] * c.y - x2[t][1] * sn.y, p.k_scale);
+        store_kv8_pair(dst + HALF + i, x2[t][0] * c.x + x1[t][0] * sn.x, x2[t][1] * c.y + x1[t][1] * sn.y, p.k_scale);
+      }
+    }
+    if (threadIdx.x == 0) trace_fine(TRF_ROPE + 1);
+    return;
+  }
   __nv_bfloat16* dst = (kind == 0) ? p.q_out + (size_t)m * H * HD + (size_t)head * HD
                                    : p.k_cache + ((size_t)slot * KV + (head - H)) * HD;
 #pragma unroll

@@ -159,8 +159,15 @@ static int launch_norm(Launcher& L, int M, int d, const NormParams& np) {
   if (slices == 2) return L.go(add_rmsnorm_kernel<2>, dim3(M), dim3(threads), 0, np);
   return L.go(add_rmsnorm_kernel<0>, dim3(M), dim3(threads), (size_t)d * 4, np);
 }
-static int launch_rope(Launcher& L, int M, const RopeParams& rp) {
+static int launch_rope(Launcher& L, int M, const RopeParams& rp, bool kv8 = false) {
   const dim3 grid(M, (rp.heads + 2 * rp.kv_heads + 3) / 4), block(128);
+  if (kv8) {  // e4m3 KV cache: the head_dims paged attention is built for
+    switch (rp.head_dim) {
+      case 64: return L.go(rope_store_kernel<64, true>, grid, block, 0, rp);
+      case 128: return L.go(rope_store_kernel<128, true>, grid, block, 0, rp);
+      default: return fail("unsupported head_dim %d for an FP8 KV cache (64 and 128 are built)", rp.head_dim);
+    }
+  }
   switch (rp.head_dim) {
     case 64: return L.go(rope_store_kernel<64>, grid, block, 0, rp);
     case 128: return L.go(rope_store_kernel<128>, grid, block, 0, rp);
@@ -266,6 +273,10 @@ struct Model {
   bf16* k_cache = nullptr;
   bf16* v_cache = nullptr;
   int64_t num_blocks = 0;
+  // ssdk_bind_kv_cache_fp8: the caches hold e4m3 codes (k_cache / v_cache then point at bytes), layer l's K = k_scale[l] *
+  // code and V = v_scale[l] * code
+  bool kv_fp8 = false;
+  std::vector<float> k_scale, v_scale;
   // derived (per TP rank)
   int H, KV, hd, d, ffn, qkv_dim, vocab_local;
 };
@@ -508,33 +519,44 @@ static int attn_plan(const Model& m, int B, int Q, int* TQ, int* MT, int* nqt, i
   return attn_plan_raw(m.H, m.KV, B, Q, max_ctx, TQ, MT, nqt, nsplit);
 }
 
-template <int HD, int MT>
+template <int HD, int MT, bool KV8>
 static int launch_attn_inst(Launcher& L, const AttnParams& p, const AttnVarlen* var, dim3 grid) {
-  const size_t smem = (size_t)2 * 2 * kAttChunk * (HD + 8) * 2;
+  const size_t smem = (size_t)attn_smem_bytes(HD);
   static bool attr_set = false;
   if (!attr_set) {
-    CK(cudaFuncSetAttribute(paged_attn_kernel<HD, MT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    CK(cudaFuncSetAttribute(paged_attn_varlen_kernel<HD, MT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CK(cudaFuncSetAttribute(paged_attn_kernel<HD, MT, KV8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CK(cudaFuncSetAttribute(paged_attn_varlen_kernel<HD, MT, KV8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr_set = true;
   }
-  if (var) return L.go(paged_attn_varlen_kernel<HD, MT>, grid, dim3(attn_warps(MT) * 32), smem, p, *var);
-  return L.go(paged_attn_kernel<HD, MT>, grid, dim3(attn_warps(MT) * 32), smem, p);
+  if (var) return L.go(paged_attn_varlen_kernel<HD, MT, KV8>, grid, dim3(attn_warps(MT) * 32), smem, p, *var);
+  return L.go(paged_attn_kernel<HD, MT, KV8>, grid, dim3(attn_warps(MT) * 32), smem, p);
 }
-static int launch_attn(Launcher& L, const AttnParams& p, const AttnVarlen* var, int hd, int MT, dim3 grid) {
-  if (hd == 128 && MT == 1) return launch_attn_inst<128, 1>(L, p, var, grid);
-  if (hd == 128 && MT == 2) return launch_attn_inst<128, 2>(L, p, var, grid);
-  if (hd == 128 && MT == 4) return launch_attn_inst<128, 4>(L, p, var, grid);
-  if (hd == 64 && MT == 1) return launch_attn_inst<64, 1>(L, p, var, grid);
-  if (hd == 64 && MT == 2) return launch_attn_inst<64, 2>(L, p, var, grid);
-  if (hd == 64 && MT == 4) return launch_attn_inst<64, 4>(L, p, var, grid);
+template <bool KV8>
+static int launch_attn_kv(Launcher& L, const AttnParams& p, const AttnVarlen* var, int hd, int MT, dim3 grid) {
+  if (hd == 128 && MT == 1) return launch_attn_inst<128, 1, KV8>(L, p, var, grid);
+  if (hd == 128 && MT == 2) return launch_attn_inst<128, 2, KV8>(L, p, var, grid);
+  if (hd == 128 && MT == 4) return launch_attn_inst<128, 4, KV8>(L, p, var, grid);
+  if (hd == 64 && MT == 1) return launch_attn_inst<64, 1, KV8>(L, p, var, grid);
+  if (hd == 64 && MT == 2) return launch_attn_inst<64, 2, KV8>(L, p, var, grid);
+  if (hd == 64 && MT == 4) return launch_attn_inst<64, 4, KV8>(L, p, var, grid);
   return fail("unsupported head_dim %d (64 and 128 are built)", hd);
 }
+static int launch_attn(Launcher& L, const AttnParams& p, const AttnVarlen* var, int hd, int MT, dim3 grid, bool kv8) {
+  return kv8 ? launch_attn_kv<true>(L, p, var, hd, MT, grid) : launch_attn_kv<false>(L, p, var, hd, MT, grid);
+}
+
+// The cache dtype of one attention call: kv8 = e4m3 caches (kc / vc point at bytes) with K = k_scale * code and
+// V = v_scale * code.  The launch plan does not depend on it.
+struct KvDtype {
+  bool kv8 = false;
+  float k_scale = 1.f, v_scale = 1.f;
+};
 
 static int enqueue_attention(Launcher& L, const bf16* q, const bf16* kc, const bf16* vc, const int32_t* bt,
                              const int32_t* ctx_lens, bf16* out, float* part_o, float* part_lse, unsigned* counters,
                              int B, int Q, int H,
                              int KV, int hd, int block_size, int max_blocks, float scale, int TQ, int MT, int nqt,
-                             int nsplit, const VarlenFwd* var = nullptr) {
+                             int nsplit, const VarlenFwd* var = nullptr, KvDtype kvd = KvDtype{}) {
   AttnParams a;
   a.q = q; a.k_cache = kc; a.v_cache = vc; a.block_tables = bt; a.context_lens = ctx_lens; a.out = out;
   a.part_o = part_o; a.part_lse = part_lse;
@@ -543,12 +565,17 @@ static int enqueue_attention(Launcher& L, const bf16* q, const bf16* kc, const b
   a.n_split = nsplit; a.TQ = TQ; a.n_qtiles = nqt;
   a.g_shift = attn_g_shift(H, KV);
   a.scale_log2 = scale * 1.4426950408889634f;
+  a.v_scale = 1.f;
+  if (kvd.kv8) {
+    a.scale_log2 *= kvd.k_scale;
+    a.v_scale = kvd.v_scale;
+  }
   if (var) {
-    CKI(launch_attn(L, a, &var->attn, hd, MT, dim3(KV, nsplit, var->n_tiles)));
+    CKI(launch_attn(L, a, &var->attn, hd, MT, dim3(KV, nsplit, var->n_tiles), kvd.kv8));
     if (nsplit > 1) CKI(L.go(attn_combine_kernel<true>, dim3(var->M * H), dim3(32), 0, a, hd, var->attn));
     return 0;
   }
-  CKI(launch_attn(L, a, nullptr, hd, MT, dim3(KV, nsplit, B * nqt)));
+  CKI(launch_attn(L, a, nullptr, hd, MT, dim3(KV, nsplit, B * nqt), kvd.kv8));
   if (nsplit > 1) CKI(L.go(attn_combine_kernel<false>, dim3(B * Q * H), dim3(32), 0, a, hd, AttnVarlen{}));
   return 0;
 }
@@ -758,15 +785,23 @@ static int enqueue_forward(ssdk_engine* e, Launcher& L, const Fwd& f) {
     rp.k_norm_w = m.cfg.qk_norm ? lw.k_norm : nullptr;
     rp.norm_eps = m.cfg.rms_eps;
     rp.q_out = w.q;
-    rp.k_cache = m.k_cache + (size_t)l * cache_layer_stride;
-    rp.v_cache = m.v_cache + (size_t)l * cache_layer_stride;
+    KvDtype kvd;
+    if (m.kv_fp8) {  // e4m3 caches: a layer is cache_layer_stride bytes
+      rp.k_cache = reinterpret_cast<bf16*>(reinterpret_cast<uint8_t*>(m.k_cache) + (size_t)l * cache_layer_stride);
+      rp.v_cache = reinterpret_cast<bf16*>(reinterpret_cast<uint8_t*>(m.v_cache) + (size_t)l * cache_layer_stride);
+      kvd.kv8 = true; kvd.k_scale = m.k_scale[l]; kvd.v_scale = m.v_scale[l];
+    } else {
+      rp.k_cache = m.k_cache + (size_t)l * cache_layer_stride;
+      rp.v_cache = m.v_cache + (size_t)l * cache_layer_stride;
+    }
     rp.heads = m.H; rp.kv_heads = m.KV; rp.head_dim = m.hd;
-    CKI(launch_rope(L, M, rp));
+    rp.k_scale = kvd.k_scale; rp.v_scale = kvd.v_scale;
+    CKI(launch_rope(L, M, rp, kvd.kv8));
 
     // ---- attention over the paged cache ----
     CKI(enqueue_attention(L, w.q, rp.k_cache, rp.v_cache, f.block_tables, w.context_lens, w.attn_out, w.att_o,
                           w.att_lse, w.att_counters, f.B, f.Q, m.H, m.KV, m.hd, bs, mb, scale, TQ, MT, nqt, nsplit,
-                          f.var));
+                          f.var, kvd));
 
     // ---- output projection (row-parallel) ----
     const bool fuse_pub = use_symm && fused_publish_enabled() && M <= 64;
@@ -1183,12 +1218,14 @@ static int init_kernel_attrs() {
   SSDK_ATTR_G(128, EPI_BF16) SSDK_ATTR_G(128, EPI_PARTIAL) SSDK_ATTR_G(128, EPI_SILU)
   SSDK_ATTR_G(256, EPI_BF16) SSDK_ATTR_G(256, EPI_PARTIAL) SSDK_ATTR_G(256, EPI_SILU)
 #undef SSDK_ATTR_G
-#define SSDK_ATTR_A(HD, MT) \
-  CK(cudaFuncSetAttribute(paged_attn_kernel<HD, MT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * 2 * kAttChunk * (HD + 8) * 2));
+#define SSDK_ATTR_A(HD, MT)                                                                                      \
+  CK(cudaFuncSetAttribute(paged_attn_kernel<HD, MT, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, attn_smem_bytes(HD))); \
+  CK(cudaFuncSetAttribute(paged_attn_kernel<HD, MT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, attn_smem_bytes(HD)));
   SSDK_ATTR_A(128, 1) SSDK_ATTR_A(128, 2) SSDK_ATTR_A(128, 4) SSDK_ATTR_A(64, 1) SSDK_ATTR_A(64, 2) SSDK_ATTR_A(64, 4)
 #undef SSDK_ATTR_A
-#define SSDK_ATTR_AV(HD, MT) \
-  CK(cudaFuncSetAttribute(paged_attn_varlen_kernel<HD, MT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * 2 * kAttChunk * (HD + 8) * 2));
+#define SSDK_ATTR_AV(HD, MT)                                                                                     \
+  CK(cudaFuncSetAttribute(paged_attn_varlen_kernel<HD, MT, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, attn_smem_bytes(HD))); \
+  CK(cudaFuncSetAttribute(paged_attn_varlen_kernel<HD, MT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, attn_smem_bytes(HD)));
   SSDK_ATTR_AV(128, 1) SSDK_ATTR_AV(128, 2) SSDK_ATTR_AV(128, 4) SSDK_ATTR_AV(64, 1) SSDK_ATTR_AV(64, 2) SSDK_ATTR_AV(64, 4)
 #undef SSDK_ATTR_AV
   CK(cudaFuncSetAttribute(add_rmsnorm_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
@@ -1366,6 +1403,28 @@ int ssdk_bind_kv_cache(ssdk_handle h, int which, void* kv_base, int64_t num_bloc
   m.num_blocks = num_blocks;
   m.k_cache = (bf16*)kv_base;
   m.v_cache = m.k_cache + (size_t)m.cfg.layers * num_blocks * h->rt.block_size * m.KV * m.hd;
+  m.kv_fp8 = false;
+  return 0;
+}
+
+int ssdk_bind_kv_cache_fp8(ssdk_handle h, int which, void* kv_base, int64_t num_blocks, const float* k_scale,
+                           const float* v_scale) {
+  if (!h || which < 0 || which > 1 || !h->model[which].present) return fail("bind_kv_cache_fp8: bad handle/model");
+  if (which != SSDK_TARGET) return fail("bind_kv_cache_fp8: only the target's KV cache can be FP8 (the draft's stays bf16)");
+  if (h->finalized) return fail("bind_kv_cache_fp8: the engine is already finalized");
+  Model& m = h->model[which];
+  if (!kv_base || num_blocks < 1 || !k_scale || !v_scale) return fail("bind_kv_cache_fp8: bad arguments");
+  if (m.hd != 64 && m.hd != 128) return fail("bind_kv_cache_fp8: head_dim %d (64 and 128 are built)", m.hd);
+  if (((uintptr_t)kv_base & 15) != 0) return fail("bind_kv_cache_fp8: cache pointer not 16-byte aligned");
+  for (int l = 0; l < m.cfg.layers; ++l)
+    if (!(std::isfinite(k_scale[l]) && k_scale[l] > 0.f && std::isfinite(v_scale[l]) && v_scale[l] > 0.f))
+      return fail("bind_kv_cache_fp8: layer %d scales k=%g v=%g (finite and > 0 required)", l, k_scale[l], v_scale[l]);
+  m.num_blocks = num_blocks;
+  m.k_cache = (bf16*)kv_base;
+  m.v_cache = (bf16*)((uint8_t*)kv_base + (size_t)m.cfg.layers * num_blocks * h->rt.block_size * m.KV * m.hd);
+  m.k_scale.assign(k_scale, k_scale + m.cfg.layers);
+  m.v_scale.assign(v_scale, v_scale + m.cfg.layers);
+  m.kv_fp8 = true;
   return 0;
 }
 
@@ -1828,6 +1887,30 @@ int ssdk_rope_store_kv(const void* qkv, const int64_t* positions, const int32_t*
   return launch_rope(L, M, rp);
 }
 
+static int check_kv_scales(const char* what, float k_scale, float v_scale) {
+  if (!(std::isfinite(k_scale) && k_scale > 0.f && std::isfinite(v_scale) && v_scale > 0.f))
+    return fail("%s: scales k=%g v=%g (finite and > 0 required)", what, k_scale, v_scale);
+  return 0;
+}
+
+int ssdk_rope_store_kv_fp8(const void* qkv, const int64_t* positions, const int32_t* slot_mapping, const float* rope_table,
+                           const void* q_norm_w, const void* k_norm_w, float norm_eps, void* q_out, void* k_cache,
+                           void* v_cache, int M, int heads, int kv_heads, int head_dim, float k_scale, float v_scale,
+                           void* stream) {
+  CKI(check_kv_scales("rope_store_kv_fp8", k_scale, v_scale));
+  Launcher L;
+  L.st = (cudaStream_t)stream;
+  RopeParams rp;
+  rp.qkv.dense = (const bf16*)qkv; rp.qkv.partial = nullptr; rp.qkv.S = 0; rp.qkv.M = M;
+  rp.qkv.N = (heads + 2 * kv_heads) * head_dim;
+  rp.positions = positions; rp.slot_mapping = slot_mapping; rp.rope_table = rope_table;
+  rp.q_norm_w = (const bf16*)q_norm_w; rp.k_norm_w = (const bf16*)k_norm_w; rp.norm_eps = norm_eps;
+  rp.q_out = (bf16*)q_out; rp.k_cache = (bf16*)k_cache; rp.v_cache = (bf16*)v_cache;
+  rp.heads = heads; rp.kv_heads = kv_heads; rp.head_dim = head_dim;
+  rp.k_scale = k_scale; rp.v_scale = v_scale;
+  return launch_rope(L, M, rp, true);
+}
+
 int ssdk_silu_mul(const void* gate_up, void* out, int M, int ffn, void* stream) {
   if (ffn % 8) return fail("silu_mul: ffn %% 8 != 0");
   Launcher L;
@@ -1847,9 +1930,10 @@ int64_t ssdk_paged_attn_scratch_bytes(int batch, int q_len, int heads, int head_
   return (int64_t)batch * q_len * heads * kAttnMaxSplit * (head_dim + 1) * 4 + 1024 + 16384;
 }
 
-int ssdk_paged_attn(const void* q, const void* k_cache, const void* v_cache, const int32_t* block_tables,
-                    const int32_t* context_lens, void* out, void* scratch, int batch, int q_len, int heads, int kv_heads,
-                    int head_dim, int block_size, int max_blocks_per_seq, float scale, void* stream) {
+static int paged_attn_op(const void* q, const void* k_cache, const void* v_cache, const int32_t* block_tables,
+                         const int32_t* context_lens, void* out, void* scratch, int batch, int q_len, int heads,
+                         int kv_heads, int head_dim, int block_size, int max_blocks_per_seq, float scale, void* stream,
+                         KvDtype kvd) {
   if (batch * q_len > kMaxTokens) return fail("paged_attn: too many query tokens");
   Launcher L;
   L.st = (cudaStream_t)stream;
@@ -1862,7 +1946,25 @@ int ssdk_paged_attn(const void* q, const void* k_cache, const void* v_cache, con
   float* part_lse = part_o + (size_t)batch * q_len * heads * kAttnMaxSplit * head_dim;
   return enqueue_attention(L, (const bf16*)q, (const bf16*)k_cache, (const bf16*)v_cache, block_tables, context_lens,
                            (bf16*)out, part_o, part_lse, (unsigned*)scratch, batch, q_len, heads, kv_heads, head_dim, block_size,
-                           max_blocks_per_seq, scale, TQ, MT, nqt, nsplit);
+                           max_blocks_per_seq, scale, TQ, MT, nqt, nsplit, nullptr, kvd);
+}
+
+int ssdk_paged_attn(const void* q, const void* k_cache, const void* v_cache, const int32_t* block_tables,
+                    const int32_t* context_lens, void* out, void* scratch, int batch, int q_len, int heads, int kv_heads,
+                    int head_dim, int block_size, int max_blocks_per_seq, float scale, void* stream) {
+  return paged_attn_op(q, k_cache, v_cache, block_tables, context_lens, out, scratch, batch, q_len, heads, kv_heads,
+                       head_dim, block_size, max_blocks_per_seq, scale, stream, KvDtype{});
+}
+
+int ssdk_paged_attn_fp8(const void* q, const void* k_cache, const void* v_cache, const int32_t* block_tables,
+                        const int32_t* context_lens, void* out, void* scratch, int batch, int q_len, int heads,
+                        int kv_heads, int head_dim, int block_size, int max_blocks_per_seq, float scale, float k_scale,
+                        float v_scale, void* stream) {
+  CKI(check_kv_scales("paged_attn_fp8", k_scale, v_scale));
+  KvDtype kvd;
+  kvd.kv8 = true; kvd.k_scale = k_scale; kvd.v_scale = v_scale;
+  return paged_attn_op(q, k_cache, v_cache, block_tables, context_lens, out, scratch, batch, q_len, heads, kv_heads,
+                       head_dim, block_size, max_blocks_per_seq, scale, stream, kvd);
 }
 
 int ssdk_paged_attn_varlen_plan(int heads, int kv_heads, int batch, const int32_t* q_lens, int max_ctx, int* out5) {
@@ -1882,10 +1984,10 @@ int ssdk_paged_attn_varlen_plan(int heads, int kv_heads, int batch, const int32_
   return 0;
 }
 
-int ssdk_paged_attn_varlen(const void* q, const void* k_cache, const void* v_cache, const int32_t* block_tables,
-                           const int32_t* context_lens, const int32_t* q_lens, void* out, void* scratch, int batch,
-                           int heads, int kv_heads, int head_dim, int block_size, int max_blocks_per_seq, float scale,
-                           void* stream) {
+static int paged_attn_varlen_op(const void* q, const void* k_cache, const void* v_cache, const int32_t* block_tables,
+                                const int32_t* context_lens, const int32_t* q_lens, void* out, void* scratch, int batch,
+                                int heads, int kv_heads, int head_dim, int block_size, int max_blocks_per_seq,
+                                float scale, void* stream, KvDtype kvd) {
   int plan[5];
   CKI(ssdk_paged_attn_varlen_plan(heads, kv_heads, batch, q_lens, block_size * max_blocks_per_seq, plan));
   Launcher L;
@@ -1907,7 +2009,27 @@ int ssdk_paged_attn_varlen(const void* q, const void* k_cache, const void* v_cac
   float* part_lse = part_o + (size_t)var.M * heads * kAttnMaxSplit * head_dim;
   return enqueue_attention(L, (const bf16*)q, (const bf16*)k_cache, (const bf16*)v_cache, block_tables, context_lens,
                            (bf16*)out, part_o, part_lse, nullptr, batch, 0, heads, kv_heads, head_dim, block_size,
-                           max_blocks_per_seq, scale, var.plan.TQ, var.plan.MT, var.plan.n_qtiles, var.plan.n_split, &var);
+                           max_blocks_per_seq, scale, var.plan.TQ, var.plan.MT, var.plan.n_qtiles, var.plan.n_split, &var,
+                           kvd);
+}
+
+int ssdk_paged_attn_varlen(const void* q, const void* k_cache, const void* v_cache, const int32_t* block_tables,
+                           const int32_t* context_lens, const int32_t* q_lens, void* out, void* scratch, int batch,
+                           int heads, int kv_heads, int head_dim, int block_size, int max_blocks_per_seq, float scale,
+                           void* stream) {
+  return paged_attn_varlen_op(q, k_cache, v_cache, block_tables, context_lens, q_lens, out, scratch, batch, heads,
+                              kv_heads, head_dim, block_size, max_blocks_per_seq, scale, stream, KvDtype{});
+}
+
+int ssdk_paged_attn_varlen_fp8(const void* q, const void* k_cache, const void* v_cache, const int32_t* block_tables,
+                               const int32_t* context_lens, const int32_t* q_lens, void* out, void* scratch, int batch,
+                               int heads, int kv_heads, int head_dim, int block_size, int max_blocks_per_seq,
+                               float scale, float k_scale, float v_scale, void* stream) {
+  CKI(check_kv_scales("paged_attn_varlen_fp8", k_scale, v_scale));
+  KvDtype kvd;
+  kvd.kv8 = true; kvd.k_scale = k_scale; kvd.v_scale = v_scale;
+  return paged_attn_varlen_op(q, k_cache, v_cache, block_tables, context_lens, q_lens, out, scratch, batch, heads,
+                              kv_heads, head_dim, block_size, max_blocks_per_seq, scale, stream, kvd);
 }
 
 int ssdk_sample(const void* logits, int64_t ld, const float* temps, int B, int V, uint64_t seed, uint64_t step_id,

@@ -51,6 +51,7 @@ SIGNATURES: dict[str, tuple] = {
     "ssdk_bind_weight": (C.c_int, [VP, C.c_int, C.c_int, C.c_int, VP, C.c_int64, C.c_int64]),
     "ssdk_bind_weight_fp8": (C.c_int, [VP, C.c_int, C.c_int, C.c_int, VP, VP, C.c_int64, C.c_int64]),
     "ssdk_bind_kv_cache": (C.c_int, [VP, C.c_int, VP, C.c_int64]),
+    "ssdk_bind_kv_cache_fp8": (C.c_int, [VP, C.c_int, VP, C.c_int64, c_f32p, c_f32p]),
     "ssdk_workspace_bytes": (C.c_int64, [VP]),
     "ssdk_bind_workspace": (C.c_int, [VP, VP, C.c_int64]),
     "ssdk_set_nccl_comm": (C.c_int, [VP, VP]),
@@ -80,6 +81,8 @@ SIGNATURES: dict[str, tuple] = {
     "ssdk_rmsnorm": (C.c_int, [VP, VP, VP, C.c_float, VP, VP, C.c_int, C.c_int, VP]),
     "ssdk_rope_store_kv": (C.c_int, [VP, VP, VP, VP, VP, VP, C.c_float, VP, VP, VP, C.c_int, C.c_int, C.c_int,
                                      C.c_int, VP]),
+    "ssdk_rope_store_kv_fp8": (C.c_int, [VP, VP, VP, VP, VP, VP, C.c_float, VP, VP, VP, C.c_int, C.c_int, C.c_int,
+                                         C.c_int, C.c_float, C.c_float, VP]),
     "ssdk_silu_mul": (C.c_int, [VP, VP, C.c_int, C.c_int, VP]),
     "ssdk_paged_attn_scratch_bytes": (C.c_int64, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
     "ssdk_paged_attn": (C.c_int, [VP, VP, VP, VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
@@ -88,6 +91,10 @@ SIGNATURES: dict[str, tuple] = {
     "ssdk_paged_attn_varlen": (C.c_int, [VP, VP, VP, VP, VP, c_i32p, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                          C.c_int, C.c_float, VP]),
     "ssdk_paged_attn_varlen_plan": (C.c_int, [C.c_int, C.c_int, C.c_int, c_i32p, C.c_int, c_i32p]),
+    "ssdk_paged_attn_fp8": (C.c_int, [VP, VP, VP, VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                      C.c_int, C.c_float, C.c_float, C.c_float, VP]),
+    "ssdk_paged_attn_varlen_fp8": (C.c_int, [VP, VP, VP, VP, VP, c_i32p, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int,
+                                             C.c_int, C.c_int, C.c_float, C.c_float, C.c_float, VP]),
     "ssdk_sample": (C.c_int, [VP, C.c_int64, VP, C.c_int, C.c_int, C.c_uint64, C.c_uint64, VP, VP]),
     "ssdk_verify_scratch_bytes": (C.c_int64, [C.c_int, C.c_int]),
     "ssdk_verify": (C.c_int, [VP, VP, VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_uint64, C.c_uint64,

@@ -12,7 +12,7 @@ import os
 import torch
 
 from . import lib as L
-from .quant import FP8_LINEARS, quantize_layers_
+from .quant import FP8_LINEARS, quantize_layers_, resolve_kv_scales
 from .runner import ModelSpec, PairRunner
 
 
@@ -33,13 +33,15 @@ _LINEAR_LEAVES = {
 
 
 def load_safetensors_weights(path: str, spec: ModelSpec, device, tp_size: int = 1, tp_rank: int = 0,
-                             allow_fp8: bool = True) -> dict:
+                             allow_fp8: bool = True, kv_scales: bool = False) -> dict:
     """Packed per-rank weights.  bf16 / fp16 / fp32 tensors are loaded as bf16.  A float8_e4m3fn decoder linear
     `<proj>.weight` stays e4m3 and pairs with `<proj>.weight_scale` (fp32 or bf16, shape [N, 1], [N], [1] or []); the
     packed matrix then gets fp32 per-row scales lw[name + "_scale"] (a per-tensor scale is broadcast to its rows, so
     q|k|v and gate|up with different per-tensor scales become one per-row vector).  `input_scale` / `input_scale_ub`
     are activation scales of W8A8 kernels and are ignored (listed in w["ignored"]).  Block-wise scales
-    (`weight_scale_inv`) raise NotImplementedError, and so does any FP8 tensor when allow_fp8 is False."""
+    (`weight_scale_inv`) raise NotImplementedError, and so does any FP8 tensor when allow_fp8 is False.
+    kv_scales: the scalar KV cache scales `model.layers.{i}.self_attn.k_scale` / `.v_scale` are read as fp32 into
+    w["kv_scales"] (resolve_kv_scales); without it they are dropped, as every tensor the engine does not use."""
     from safetensors import safe_open
 
     H, KV, hd = spec.heads // tp_size, spec.kv_heads // tp_size, spec.head_dim
@@ -54,6 +56,7 @@ def load_safetensors_weights(path: str, spec: ModelSpec, device, tp_size: int = 
     rank_rows = {"qkv": [H * hd, KV * hd, KV * hd], "gate_up": [ffn, ffn], "o": [d], "down": [d]}
     shape = {"qkv": ((H + 2 * KV) * hd, d), "gate_up": (2 * ffn, d), "o": (d, H * hd), "down": (d, ffn)}
     scales_seen: dict[tuple[int, str, int], bool] = {}
+    kv_found: dict[tuple[str, int], float] = {}
 
     def rows(t, n):  # column-parallel: shard output rows
         return t[tp_rank * n:(tp_rank + 1) * n]
@@ -105,6 +108,13 @@ def load_safetensors_weights(path: str, spec: ModelSpec, device, tp_size: int = 
                     ignored.append(name)  # activation scales: the FP8 path is weight-only
                     continue
                 t = f.get_tensor(name)
+                if kv_scales and name.startswith("model.layers.") and name.endswith((".self_attn.k_scale",
+                                                                                     ".self_attn.v_scale")):
+                    if t.numel() != 1:
+                        raise ValueError(f"{path}: {name} has {t.numel()} elements; KV cache scales are per layer "
+                                         "(one scalar)")
+                    kv_found[(name[-7], int(name.split(".")[2]))] = float(t.to(torch.float32).reshape(-1)[0])
+                    continue
                 if t.dtype == f8 and not allow_fp8:
                     raise NotImplementedError(f"{path}: {name} is FP8 and allow_fp8=False asks for bf16 weights; FP8 "
                                               "decoder linears load for the draft as well, not for the target model "
@@ -148,6 +158,8 @@ def load_safetensors_weights(path: str, spec: ModelSpec, device, tp_size: int = 
         w["lm_head"] = w["embed"]
     if ignored:
         w["ignored"] = ignored
+    if kv_scales:
+        w["kv_scales"] = resolve_kv_scales(kv_found, spec.layers, path)
     return w
 
 
@@ -200,21 +212,28 @@ def tp_row_amax_max(amax: torch.Tensor) -> torch.Tensor:
 
 
 def load_weights(path: str, spec: ModelSpec, device, tp_size: int = 1, tp_rank: int = 0,
-                 quantization: str | None = None, is_target: bool = True) -> dict:
+                 quantization: str | None = None, is_target: bool = True, kv_cache_dtype: str = "auto") -> dict:
     """Packed per-rank weights of a synthetic directory or a safetensors checkpoint.  quantization="fp8" replaces the
     decoder linears by e4m3 + per-row scales (quant.py) after loading, one tensor at a time; FP8 checkpoint tensors are
     kept as they are either way.  With tp_size > 1 every rank must call this together: the row scales of o / down come
     from the full rows (a MAX all-reduce over the ranks' column shards).  The draft (is_target=False) is a tp = 1
-    replica on rank 0, so its rows are whole and need no reduction."""
+    replica on rank 0, so its rows are whole and need no reduction.
+    kv_cache_dtype="fp8" (target only): w["kv_scales"] = (k_scale, v_scale), per-layer lists of floats from the
+    checkpoint (1.0 without them; the same on every tensor-parallel rank)."""
     if not is_target and tp_size != 1:
         raise ValueError("the draft is loaded whole (tp_size = 1) on rank 0")
+    if not is_target and kv_cache_dtype != "auto":
+        raise ValueError("only the target's KV cache can be FP8; the draft's stays bf16")
+    kv8 = kv_cache_dtype == "fp8"
     marker = os.path.join(path, "ssd_b200_synthetic.json")
     if os.path.exists(marker):
         from .synth import generate_weights
         with open(marker) as f:
             w = generate_weights(spec, json.load(f), device, tp_size, tp_rank)
+        if kv8:
+            w["kv_scales"] = resolve_kv_scales({}, spec.layers, path)
     elif glob.glob(os.path.join(path, "*.safetensors")):
-        w = load_safetensors_weights(path, spec, device, tp_size, tp_rank, allow_fp8=True)
+        w = load_safetensors_weights(path, spec, device, tp_size, tp_rank, allow_fp8=True, kv_scales=kv8)
     else:
         raise FileNotFoundError(f"{path}: neither *.safetensors nor ssd_b200_synthetic.json")
     if quantization == "fp8":
@@ -243,18 +262,19 @@ class _DraftCfg:
     num_kvcache_blocks = 0
 
 
-def kv_block_bytes(config, spec: ModelSpec, tp_size: int) -> int:
-    return 2 * spec.layers * config.kvcache_block_size * (spec.kv_heads // tp_size) * spec.head_dim * 2
+def kv_block_bytes(config, spec: ModelSpec, tp_size: int, fp8: bool = False) -> int:
+    """Bytes of one KV page (K and V of every layer): 2 bytes per element, 1 for an FP8 (e4m3) cache."""
+    return 2 * spec.layers * config.kvcache_block_size * (spec.kv_heads // tp_size) * spec.head_dim * (1 if fp8 else 2)
 
 
-def kv_blocks_for(config, spec: ModelSpec, tp_size: int, share: float, reserved: int = 0) -> int:
+def kv_blocks_for(config, spec: ModelSpec, tp_size: int, share: float, reserved: int = 0, fp8: bool = False) -> int:
     """allocate_kv_cache (engine/model_runner.py:446-476): blocks that fit in share * gpu_memory_utilization * free,
     capped at what max_num_seqs sequences of max_model_len (+ prefix-cache slack) can ever use.  `reserved` = bytes
     already promised to another cache out of the same free-memory snapshot (the reference sizes the draft cache from
-    what REMAINS after the target's, draft_runner.py:27)."""
+    what REMAINS after the target's, draft_runner.py:27).  fp8: pages of an e4m3 cache (half the bytes)."""
     free, _ = torch.cuda.mem_get_info()
     free = max(0, free - reserved)
-    block_bytes = kv_block_bytes(config, spec, tp_size)
+    block_bytes = kv_block_bytes(config, spec, tp_size, fp8)
     fit = int(free * config.gpu_memory_utilization * share) // block_bytes
     want = max(config.max_num_seqs, 1) * config.max_blocks * 2 + 2
     return max(1, min(fit, want))
@@ -265,14 +285,16 @@ def build_runner(config, tp_size: int = 1, tp_rank: int = 0, device=None, finali
     torch.cuda.set_device(device)
     tspec = spec_from_config(config.hf_config)
     dspec = spec_from_config(config.draft_hf_config) if config.speculate else None
-    wt = load_weights(config.model, tspec, device, tp_size, tp_rank, quantization=config.quantization)
+    kv8 = getattr(config, "kv_cache_dtype", "auto") == "fp8"
+    wt = load_weights(config.model, tspec, device, tp_size, tp_rank, quantization=config.quantization,
+                      kv_cache_dtype="fp8" if kv8 else "auto")
     if is_fp8(wt):  # an FP8 checkpoint found by its tensor dtypes
         config.quantization = "fp8"
     wd = load_draft_weights(config, dspec, device) if (dspec is not None and tp_rank == 0) else None
     if dspec is not None and tp_rank != 0:
         dspec = None  # the draft is a replica pinned to rank 0 (SURVEY §8e)
-    nbt = kv_blocks_for(config, tspec, tp_size, 0.8 if dspec else 1.0)
-    nbd = kv_blocks_for(config, dspec, 1, 0.75, reserved=nbt * kv_block_bytes(config, tspec, tp_size)) if dspec else None
+    nbt = kv_blocks_for(config, tspec, tp_size, 0.8 if dspec else 1.0, fp8=kv8)
+    nbd = kv_blocks_for(config, dspec, 1, 0.75, reserved=nbt * kv_block_bytes(config, tspec, tp_size, kv8)) if dspec else None
     config.num_kvcache_blocks = nbt
     draft_cfg = _DraftCfg()
     draft_cfg.num_kvcache_blocks = nbd or nbt
@@ -280,7 +302,8 @@ def build_runner(config, tp_size: int = 1, tp_rank: int = 0, device=None, finali
                         max_batch=max(1, config.max_num_seqs), block_size=config.kvcache_block_size,
                         max_model_len=config.max_model_len, num_blocks_target=nbt, num_blocks_draft=nbd, device=device,
                         use_graph=config.use_cuda_graph, use_pdl=config.use_pdl, jit_speculate=config.jit_speculate,
-                        tp_size=tp_size, tp_rank=tp_rank, draft_fp8=wd is not None and is_fp8(wd))
+                        tp_size=tp_size, tp_rank=tp_rank, draft_fp8=wd is not None and is_fp8(wd),
+                        target_kv_scales=wt["kv_scales"] if kv8 else None)
     runner.bind_weights(L.TARGET, wt)
     if wd is not None:
         runner.bind_weights(L.DRAFT, wd)

@@ -152,6 +152,28 @@ def rope_store_kv(qkv: torch.Tensor, positions: torch.Tensor, slot_mapping: torc
     return q
 
 
+def rope_store_kv_fp8(qkv: torch.Tensor, positions: torch.Tensor, slot_mapping: torch.Tensor, rope_table: torch.Tensor,
+                      k_cache: torch.Tensor, v_cache: torch.Tensor, heads: int, kv_heads: int, head_dim: int,
+                      k_scale: float, v_scale: float, q_norm_w: torch.Tensor | None = None,
+                      k_norm_w: torch.Tensor | None = None, norm_eps: float = 1e-6) -> torch.Tensor:
+    """rope_store_kv into float8_e4m3fn caches: k and v are stored as e4m3_rne(clamp(y / scale, -448, 448)) of the
+    bf16 values y that rope_store_kv stores (quant.quantize_kv_fp8).  Returns q [M, H*hd] as rope_store_kv does."""
+    _req(qkv, torch.bfloat16, "qkv")
+    _req(positions, torch.int64, "positions")
+    _req(slot_mapping, torch.int32, "slot_mapping")
+    _req(rope_table, torch.float32, "rope_table")
+    _req(k_cache, torch.float8_e4m3fn, "k_cache")
+    _req(v_cache, torch.float8_e4m3fn, "v_cache")
+    M = qkv.shape[0]
+    q = torch.empty(M, heads * head_dim, dtype=torch.bfloat16, device=qkv.device)
+    lib = _L.load()
+    _L.check(lib.ssdk_rope_store_kv_fp8(_ptr(qkv), _ptr(positions), _ptr(slot_mapping), _ptr(rope_table), _ptr(q_norm_w),
+                                        _ptr(k_norm_w), float(norm_eps), _ptr(q), _ptr(k_cache), _ptr(v_cache), M, heads,
+                                        kv_heads, head_dim, float(k_scale), float(v_scale), _stream()),
+             "ssdk_rope_store_kv_fp8")
+    return q
+
+
 def silu_and_mul(x: torch.Tensor) -> torch.Tensor:
     """SiluAndMul.forward (layers/activation.py:11-14)."""
     _req(x, torch.bfloat16, "x")
@@ -231,6 +253,56 @@ def paged_attention_varlen_plan(q_lens: list[int], H: int, KV: int, max_ctx: int
     lib = _L.load()
     _L.check(lib.ssdk_paged_attn_varlen_plan(H, KV, len(q_lens), ql, max_ctx, out), "ssdk_paged_attn_varlen_plan")
     return {"TQ": out[0], "MT": out[1], "n_qtiles": out[2], "n_split": out[3], "n_tiles": out[4]}
+
+
+def paged_attention_fp8(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, block_tables: torch.Tensor,
+                        context_lens: torch.Tensor, q_len: int, scale: float, k_scale: float,
+                        v_scale: float) -> torch.Tensor:
+    """paged_attention over float8_e4m3fn caches [num_blocks, block_size, KV, hd]: attention over K = k_scale * code and
+    V = v_scale * code, with the plan paged_attention takes for the same sizes."""
+    _req(q, torch.bfloat16, "q")
+    _req(k_cache, torch.float8_e4m3fn, "k_cache")
+    _req(v_cache, torch.float8_e4m3fn, "v_cache")
+    _req(block_tables, torch.int32, "block_tables")
+    _req(context_lens, torch.int32, "context_lens")
+    Mq, H, hd = q.shape
+    B = Mq // q_len
+    _, block_size, KV, _ = k_cache.shape
+    max_blocks = block_tables.shape[1]
+    lib = _L.load()
+    nbytes = lib.ssdk_paged_attn_scratch_bytes(B, q_len, H, hd, max_blocks * block_size)
+    scratch = torch.empty(nbytes, dtype=torch.uint8, device=q.device)
+    out = torch.empty(Mq, H * hd, dtype=torch.bfloat16, device=q.device)
+    _L.check(lib.ssdk_paged_attn_fp8(_ptr(q), _ptr(k_cache), _ptr(v_cache), _ptr(block_tables), _ptr(context_lens),
+                                     _ptr(out), _ptr(scratch), B, q_len, H, KV, hd, block_size, max_blocks, float(scale),
+                                     float(k_scale), float(v_scale), _stream()), "ssdk_paged_attn_fp8")
+    return out
+
+
+def paged_attention_varlen_fp8(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor,
+                               block_tables: torch.Tensor, context_lens: torch.Tensor, q_lens: list[int], scale: float,
+                               k_scale: float, v_scale: float) -> torch.Tensor:
+    """paged_attention_varlen over float8_e4m3fn caches (K = k_scale * code, V = v_scale * code)."""
+    _req(q, torch.bfloat16, "q")
+    _req(k_cache, torch.float8_e4m3fn, "k_cache")
+    _req(v_cache, torch.float8_e4m3fn, "v_cache")
+    _req(block_tables, torch.int32, "block_tables")
+    _req(context_lens, torch.int32, "context_lens")
+    Mq, H, hd = q.shape
+    B = len(q_lens)
+    assert sum(q_lens) == Mq and context_lens.shape[0] == B and block_tables.shape[0] == B
+    _, block_size, KV, _ = k_cache.shape
+    max_blocks = block_tables.shape[1]
+    ql = (C.c_int32 * B)(*q_lens)
+    lib = _L.load()
+    nbytes = lib.ssdk_paged_attn_scratch_bytes(1, Mq, H, hd, max_blocks * block_size)
+    scratch = torch.empty(nbytes, dtype=torch.uint8, device=q.device)
+    out = torch.empty(Mq, H * hd, dtype=torch.bfloat16, device=q.device)
+    _L.check(lib.ssdk_paged_attn_varlen_fp8(_ptr(q), _ptr(k_cache), _ptr(v_cache), _ptr(block_tables),
+                                            _ptr(context_lens), ql, _ptr(out), _ptr(scratch), B, H, KV, hd, block_size,
+                                            max_blocks, float(scale), float(k_scale), float(v_scale), _stream()),
+             "ssdk_paged_attn_varlen_fp8")
+    return out
 
 
 def sample(logits: torch.Tensor, temperatures: torch.Tensor, seed: int = 0, step_id: int = 0) -> torch.Tensor:

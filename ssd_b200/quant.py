@@ -11,6 +11,8 @@ The quantization runs on whatever device the tensor is on, one tensor at a time,
 matrix by its FP8 form as it goes never holds a second copy of the model."""
 from __future__ import annotations
 
+import math
+
 import torch
 
 E4M3_MAX = 448.0
@@ -79,6 +81,42 @@ def checkpoint_quantization(hf) -> str | None:
                                               "supported: per-channel or per-tensor scales only")
                 return "fp8"
     raise NotImplementedError(f"quantization_config {qc!r}: only FP8 (e4m3) weight checkpoints are supported")
+
+
+def parse_kv_cache_dtype(v: str) -> str:
+    """Config.kv_cache_dtype -> "auto" (bf16 KV cache) or "fp8" (e4m3 target KV cache with per-layer scales)."""
+    if v in ("auto", "bf16", "bfloat16"):
+        return "auto"
+    if v in ("fp8", "fp8_e4m3"):
+        return "fp8"
+    if v == "fp8_e5m2":
+        raise NotImplementedError("kv_cache_dtype='fp8_e5m2' is not supported: the FP8 KV cache is e4m3 ('fp8')")
+    raise ValueError(f"kv_cache_dtype={v!r}: supported values are 'auto' / 'bf16' / 'bfloat16' (bf16 KV cache) and "
+                     "'fp8' / 'fp8_e4m3' (float8 e4m3 target KV cache)")
+
+
+def quantize_kv_fp8(y: torch.Tensor, scale: float) -> torch.Tensor:
+    """The FP8 KV store (ssdk_bind_kv_cache_fp8): e4m3_rne(clamp(y / scale, -448, 448)) of the bf16 values y, divided
+    tensor by tensor (IEEE fp32 division on any device)."""
+    yf = y.float()
+    return (yf / torch.full_like(yf, scale)).clamp(-E4M3_MAX, E4M3_MAX).to(torch.float8_e4m3fn)
+
+
+def resolve_kv_scales(found: dict[tuple[str, int], float], layers: int, where: str = "checkpoint"
+                      ) -> tuple[list[float], list[float]]:
+    """Per-layer (k_scale, v_scale) of an FP8 KV cache from the checkpoint's `model.layers.{i}.self_attn.k_scale` /
+    `.v_scale` scalars (found[("k" | "v", i)]): all 1.0 when there are none.  Scales on some layers only, or a scale
+    that is not finite or not > 0, raise ValueError."""
+    if not found:
+        return [1.0] * layers, [1.0] * layers
+    missing = [f"{kind}_scale of layer {i}" for i in range(layers) for kind in ("k", "v") if (kind, i) not in found]
+    if missing:
+        raise ValueError(f"{where}: KV cache scales on some layers only (missing {', '.join(missing[:4])}"
+                         f"{', ...' if len(missing) > 4 else ''})")
+    for (kind, i), s in sorted(found.items()):
+        if not (math.isfinite(s) and s > 0):
+            raise ValueError(f"{where}: layer {i} {kind}_scale = {s!r}: KV cache scales must be finite and > 0")
+    return [found[("k", i)] for i in range(layers)], [found[("v", i)] for i in range(layers)]
 
 
 def parse_quantization(q: str | None) -> str | None:

@@ -69,7 +69,9 @@ class PairRunner:
                  block_size: int = 256, max_model_len: int = 4096, num_blocks_target: int | None = None,
                  num_blocks_draft: int | None = None, device: str | torch.device = "cuda:0", use_graph: bool = True,
                  use_pdl: bool = False, jit_speculate: bool = True, tp_size: int = 1, tp_rank: int = 0,
-                 draft_fp8: bool = False):
+                 draft_fp8: bool = False, target_kv_scales: tuple[list[float], list[float]] | None = None):
+        """target_kv_scales: (k_scale, v_scale) per target layer for an FP8 (e4m3) target KV cache, bound with
+        ssdk_bind_kv_cache_fp8; None keeps it bf16.  The draft's cache is always bf16."""
         if not torch.cuda.is_available():
             raise RuntimeError("PairRunner needs a CUDA device: libssdk has no CPU path")
         self.lib = L.load()
@@ -97,14 +99,25 @@ class PairRunner:
         self.h = h
         # KV caches: [2, L, num_blocks, block_size, KV/tp, hd] (engine/model_runner.py:484-491)
         self.kv = {}
+        self.kv_scales = None  # (k_scale, v_scale) lists of an FP8 target cache
         for which, m, nb, tp in ((L.TARGET, target, num_blocks_target, tp_size), (L.DRAFT, draft, num_blocks_draft, 1)):
             if m is None:
                 continue
             nb = nb or max_batch * self.max_blocks
-            kv = torch.zeros(2, m.layers, nb, block_size, m.kv_heads // tp, m.head_dim, dtype=torch.bfloat16,
-                             device=self.device)
-            self.kv[which] = kv
-            L.check(self.lib.ssdk_bind_kv_cache(self.h, which, kv.data_ptr(), nb), "ssdk_bind_kv_cache")
+            shape = (2, m.layers, nb, block_size, m.kv_heads // tp, m.head_dim)
+            if which == L.TARGET and target_kv_scales is not None:
+                ks, vs = (np.ascontiguousarray(s, dtype=np.float32) for s in target_kv_scales)
+                if ks.shape != (m.layers,) or vs.shape != (m.layers,):
+                    raise ValueError(f"target_kv_scales: {m.layers} k and v scales expected")
+                kv = torch.zeros(shape, dtype=torch.uint8, device=self.device).view(torch.float8_e4m3fn)
+                self.kv[which] = kv
+                self.kv_scales = (ks.tolist(), vs.tolist())
+                L.check(self.lib.ssdk_bind_kv_cache_fp8(self.h, which, kv.data_ptr(), nb, ks.ctypes.data_as(L.c_f32p),
+                                                        vs.ctypes.data_as(L.c_f32p)), "ssdk_bind_kv_cache_fp8")
+            else:
+                kv = torch.zeros(*shape, dtype=torch.bfloat16, device=self.device)
+                self.kv[which] = kv
+                L.check(self.lib.ssdk_bind_kv_cache(self.h, which, kv.data_ptr(), nb), "ssdk_bind_kv_cache")
             table = rope_table(m.head_dim, self.max_blocks * block_size, m.rope_theta, self.device)
             self._keep.append(table)
             L.check(self.lib.ssdk_bind_weight(self.h, which, L.W_ROPE_TABLE, 0, table.data_ptr(), table.shape[0],
